@@ -6,7 +6,7 @@
 Headline workload (BASELINE.json `metric` "4K Hap-Q encode/decode GB/s per GPU", configs[2]): 3840x2160 RGBA8
 synthetic video frames -> Hap Q (scaled-YCoCg-DXT5, Snappy, 8 chunks) -> decoded back to the DXT texture bytes
 (what HapDecode returns).  One STEP = one pass of that round trip over a batch of `--frames` device-resident
-frames per GPU (default 444 = 14.7 GB of RGBA, far larger than the 126 MB L2).  `value` = RGBA bytes pushed through
+frames per GPU (default 444 = 14.7 GB of RGBA, far larger than the H100's 50 MB L2).  `value` = RGBA bytes pushed through
 the round trip per second, all GPUs together (frames are independent: ranks take disjoint frames, weak scaling).
 
 Legs outside the timed region (rank 0 / N=1 unless noted):
@@ -16,8 +16,12 @@ Legs outside the timed region (rank 0 / N=1 unless noted):
   roofline       per-stage CUDA-event timing of the headline step, dominant kernel vs the measured HBM peak
   extra.configs  encode-only and decode-only GB/s, fps and roofline fraction for every configuration of
                  BASELINE.json (1080p Hap x1, 4K Hap x1, 4K Hap Q x8, 8K Hap Q Alpha x32, 16K Hap Q x64)
-  cpu_baseline   the reference's own CPU path on this box's host cores (see reference_cpu_path)
+  cpu_baseline   the reference's own CPU path on the host's cores (see reference_cpu_path)
   extra.ref_stream_decode   decode of frames the REFERENCE encoder (hap.c + Google Snappy) made in that leg
+
+`--dump-outputs DIR` writes what the last timed step of the headline workload returned as DIR/<name>.npy (each rank into
+DIR/rank<r>/ when there are several; see dump_outputs), so that two builds can be compared output for output on identical
+inputs.
 
 `--impl reference` times only the reference's CPU path: unmodified hap.c (oracle/_ref) HapEncode frame-parallel over all
 cores + HapDecode (frame-parallel, and through its chunk callback on a pthread pool), whole 4K Hap Q 8-chunk frames.
@@ -53,7 +57,7 @@ def measured_peak_hbm():
         with open(p) as fh:
             return float(json.load(fh)["hbm_gbs"]), "measured(MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback(B200_PROFILING.md)"
+        return 3350.0, "datasheet(H100 SXM HBM3, 3.35 TB/s)"
 
 
 class ClockSampler:
@@ -230,6 +234,9 @@ def run_reference_arm(args, rank, world):
 # GPU arm
 # =====================================================================================================
 
+SYNTH_BAND_BYTES = 1 << 28
+
+
 class Roundtrip:
     """A device-resident batch of one configuration: RGBA frames, the encoded frames, the decoded textures."""
 
@@ -239,8 +246,10 @@ class Roundtrip:
         self.lib, self.dev, self.w, self.h, self.codec, self.chunks, self.F = lib, dev, w, h, codec, chunks, frames
         self.rgba_bytes = 4 * w * h
         self.rgba = torch.empty((frames, h, w, 4), dtype=torch.uint8, device=dev)
+        band = max(1, SYNTH_BAND_BYTES // (32 * w))    # rows per synth call: its int64 intermediates stay near 256 MB
         for i in range(frames):
-            self.rgba[i] = synth.frame(w, h, first_index + i, device=dev, alpha=alpha)
+            for y in range(0, h, band):
+                self.rgba[i, y:y + band] = synth.frame(w, h, first_index + i, device=dev, alpha=alpha, rows=(y, min(y + band, h)))
         self.tex_bytes = [lib.texture_bytes(w, h, codec, 0), lib.texture_bytes(w, h, codec, 1)]
         self.ntex = 2 if self.tex_bytes[1] else 1
         self.cap = (lib.max_encoded_length_rgba(w, h, codec, chunks) + 15) // 16 * 16
@@ -272,6 +281,34 @@ class Roundtrip:
 
     def mean_frame_bytes(self):
         return float(self.used.double().mean().item())
+
+
+DUMP_SAMPLE = 1 << 22   # bytes sampled from each batch-sized output (16 MiB as float32)
+
+
+def dump_outputs(path, rt, frames, used):
+    """Writes what the last timed step returned to its caller as float64 / float32 .npy files under `path`: per frame the
+    encoded length, the decode result, the decoded length and texture format in full; of the encoded frames and of each
+    decoded texture (hundreds of MB per batch) a fixed sample of DUMP_SAMPLE bytes drawn with seed 0.  Encoded bytes are
+    sampled at fixed fractions of each frame's own length, so every sampled byte lies inside a frame."""
+    import numpy as np
+    import torch
+    os.makedirs(path, exist_ok=True)
+    dev = frames.device
+    g = torch.Generator().manual_seed(0)
+    lengths = used.cpu()
+    fi = torch.randint(0, rt.F, (DUMP_SAMPLE,), generator=g)
+    pos = (torch.rand(DUMP_SAMPLE, generator=g, dtype=torch.float64) * lengths[fi].double()).long()
+    out = {"encoded_lengths": lengths.double(), "decode_results": rt.res.cpu().double(),
+           "decoded_lengths": rt.tex_used.cpu().double(), "texture_formats": rt.fmts.cpu().double(),
+           "encoded_sample": frames[(fi * rt.cap + pos).to(dev)].cpu().float()}
+    for ti in range(rt.ntex):
+        n, stride = rt.tex_bytes[ti], (rt.tex_bytes[ti] + 15) // 16 * 16
+        tf = torch.randint(0, rt.F, (DUMP_SAMPLE,), generator=g)
+        to = torch.randint(0, n, (DUMP_SAMPLE,), generator=g)
+        out[f"decoded_texture{ti}_sample"] = rt.tex[ti][(tf * stride + to).to(dev)].cpu().float()
+    for name, t in out.items():
+        np.save(os.path.join(path, name + ".npy"), t.numpy())
 
 
 def time_on_stream(torch, stream, fn, iters, warm=2):
@@ -430,6 +467,9 @@ def run_gpu_arm(args, rank, local_rank, world):
         launches = lib.launches() - launches0
         clocks = sampler.stop(wall0, wall1) if rank == 0 else None
         A.check()
+        if args.dump_outputs:
+            last = (args.steps - 1) & 1     # buffer of the last timed step; A's textures hold its decode (drain())
+            dump_outputs(args.dump_outputs if world == 1 else os.path.join(args.dump_outputs, f"rank{rank}"), A, frames_buf[last], used[last])
         ms = torch.tensor([e0.elapsed_time(e1)], dtype=torch.float64, device=dev)
         if world > 1:
             dist.all_reduce(ms, op=dist.ReduceOp.MAX)
@@ -814,7 +854,14 @@ def main():
     ap.add_argument("--profile", action="store_true", help="short run for ncu: skip the e2e, extra and CPU legs")
     ap.add_argument("--no-overlap", action="store_true", help="encode and decode of a batch back to back on one stream")
     ap.add_argument("--no-index", action="store_true", help="frames without the trailing fragment index section (decoder indexes on the fly)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs of the headline workload as DIR/<name>.npy "
+                                                            "(DIR/rank<r>/<name>.npy with more than one rank)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and (args.impl != "b200" or args.workload != "4k_hapq"):
+        ap.error("--dump-outputs writes the outputs of the GPU arm's 4k_hapq workload; it has none to write with --impl reference "
+                 "or --workload 16k_stream")
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))

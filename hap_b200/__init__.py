@@ -1,4 +1,4 @@
-"""hap_b200 -- B200-native Hap frame codec.
+"""hap_b200 -- H100-native (sm_90a) Hap frame codec.
 
 The product is the C-ABI shared library `libhap_b200.so` (sources in hap_b200/csrc, API in include/).
 This package only loads it and mirrors its entry points for Python callers (tests, bench):

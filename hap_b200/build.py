@@ -1,4 +1,4 @@
-"""Builds libhap_b200.so (sm_100a) in-tree with nvcc.  `python -m hap_b200.build`"""
+"""Builds libhap_b200.so (sm_90a, H100) in-tree with nvcc.  `python -m hap_b200.build`"""
 from __future__ import annotations
 
 import os
@@ -12,7 +12,7 @@ SRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libhap_b200.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-fmad=false",             # FMAs are written explicitly (bc_block.cuh) so the CPU twin matches bit for bit
     "-Xcompiler", "-fPIC",

@@ -84,8 +84,8 @@ __device__ __forceinline__ uint32_t hap_prmt(uint32_t a, uint32_t b, uint32_t se
 
 HAP_HD int hap_clampi(int v, int lo, int hi) { return v < lo ? lo : v > hi ? hi : v; }
 
-// Three-input min/max, clamp(a+b, 0, c) and saturate: single instructions on sm_100a (VIMNMX3, FMNMX3,
-// VIADDMNMX.RELU, FFMA.SAT); plain C++ on the host so that the CPU twin computes the same values.
+// Three-input min/max, clamp(a+b, 0, c) and saturate: CUDA intrinsics on the device (sm_90a lowers each to a few
+// IMNMX / IADD / FMNMX instructions); plain C++ on the host so that the CPU twin computes the same values.
 #if defined(HAPB200_EMU) || !defined(__CUDA_ARCH__)
 HAP_HD int hap_max3(int a, int b, int c) { int m = a > b ? a : b; return m > c ? m : c; }
 HAP_HD int hap_min3(int a, int b, int c) { int m = a < b ? a : b; return m < c ? m : c; }

@@ -84,7 +84,7 @@ constexpr int kMaxDevices = 64;
 struct DeviceState {
     std::once_flag once;
     bool ready = false;
-    int sm_count = 148;
+    int sm_count = 132;
 };
 DeviceState g_dev[kMaxDevices];
 std::atomic<int> g_default_device{-1};
@@ -94,7 +94,7 @@ thread_local int t_device = 0;   // device of the library call running on this t
 void device_init(int dev)
 {
     DeviceState &d = g_dev[dev];
-    if (cudaDeviceGetAttribute(&d.sm_count, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || d.sm_count <= 0) { cudaGetLastError(); d.sm_count = 148; }
+    if (cudaDeviceGetAttribute(&d.sm_count, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || d.sm_count <= 0) { cudaGetLastError(); d.sm_count = 132; }
     cudaMemPool_t pool;
     if (cudaDeviceGetDefaultMemPool(&pool, dev) == cudaSuccess) {
         unsigned long long keep = ~0ull;  // keep freed scratch in the pool: steady-state calls never hit the OS
@@ -587,7 +587,7 @@ __global__ void ring_wait_kernel(const unsigned int *flag, unsigned int value, u
 // =====================================================================================================
 extern "C" {
 
-const char *HapB200Version(void) { return "hap-b200 0.1 (sm_100a)"; }
+const char *HapB200Version(void) { return "hap-b200 0.1 (sm_90a)"; }
 unsigned long long HapB200KernelLaunchCount(void) { return g_launches.load(); }
 
 // The device host-pointer calls run on (device-pointer calls run where their buffers live).  -1: forget it; the next
@@ -691,7 +691,7 @@ unsigned int HapB200RingWait(int device, const void *flag, unsigned int value, u
     if (timeoutMs == 0) {
         // No timeout asked for: a stream memory operation of the driver (cuStreamWaitValue32, "flag - value >= 0" compared as
         // signed), which holds the stream WITHOUT occupying an SM.  (A polling kernel resident on one SM keeps the encoder's
-        // one-CTA-per-SM fragment kernel from getting that SM: measured, a third more time per step.)
+        // one-CTA-per-SM fragment kernel from getting that SM, so the last CTA of that grid runs as a second wave.)
         typedef int (*WaitValue32)(cudaStream_t, unsigned long long, unsigned int, unsigned int);
         static WaitValue32 wait_value = [] {
             void *fn = nullptr;

@@ -22,7 +22,7 @@ __device__ __forceinline__ hap_saddr_t hap_smem_addr(const void *p) { return (ha
 __device__ __forceinline__ uint32_t hap_lds_u8(hap_saddr_t a) { uint32_t v; asm volatile("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(a)); return v; }
 __device__ __forceinline__ void hap_sts_u16(hap_saddr_t a, uint32_t v) { asm volatile("st.shared.u16 [%0], %1;" ::"r"(a), "h"((unsigned short)v)); }
 
-// ---- sm_90+/sm_100 asynchronous bulk copies (TMA, 1-D) completed on an mbarrier ------------------------------------
+// ---- sm_90 (Hopper) asynchronous bulk copies (TMA, 1-D) completed on an mbarrier ------------------------------------
 // Global -> shared, `bytes` a multiple of 16, both addresses 16-byte aligned.  One thread issues the copy; the TMA unit
 // moves the bytes without occupying issue slots or registers and signals the mbarrier with the byte count.
 // SASS: UBLKCP (copy), SYNCS (mbarrier).  The emulator build (tests/emu/simt_emu.h) copies synchronously.

@@ -480,8 +480,9 @@ __global__ void hap_requeue_mismatched_kernel(ChunkJob *jobs, uint32_t njobs, ui
 #ifndef HAPB200_EX_MIN_BLOCKS
 #define HAPB200_EX_MIN_BLOCKS 4
 #endif
-// Measured (r02c, 444 4K Hap Q frames with index): 2048 descriptors / 32 KiB tiles / 3 CTAs per SM (74 KB, 80 registers):
-// 6.40 ms; 1024 / 16 KiB / 3 CTAs: 6.26 ms; 1024 / 16 KiB / 4 CTAs per SM (54 KB, 64 registers, no spills): 5.56 ms.
+// 1024 descriptors / 16 KiB tiles at 4 CTAs per SM (54 KB, 64 registers; sm_90a spills 108 bytes) against 3 CTAs per SM
+// (80 registers, 40 bytes of spills), this kernel's time on 444 4K Hap Q frames with index, H100 80GB HBM3 at a 400 W
+// power limit, four alternating runs each: 6.94-7.12 ms at 4, 7.07-7.43 ms at 3.  Outputs are identical.
 constexpr int kExThreads = 256;
 constexpr int kExMaxElems = HAPB200_EX_MAX_ELEMS;    // descriptors held in shared memory per pass
 constexpr int kExMaxIn = 32768 + 64;                 // stream bytes of one window the staging buffer holds

@@ -209,6 +209,6 @@ def load() -> HapB200:
     path = library_path()
     if not os.path.exists(path):
         raise RuntimeError(
-            f"{path} is missing: build it with `python -m hap_b200.build` (nvcc, sm_100a). "
+            f"{path} is missing: build it with `python -m hap_b200.build` (nvcc, sm_90a). "
             "hap_b200 has no CPU implementation to fall back to.")
     return HapB200(path)

@@ -257,10 +257,9 @@ def run(args, rank, local_rank, world, emit, ClockSampler, measured_peak_hbm):
             "value": frames_per_step * rgba_bytes / (ms_n * 1e-3) / 1e9, "nvlink_bytes_per_step": moved["bytes"],
             "nvlink_GBps_into_rank0": moved["bytes"] / (ms_n * 1e-3) / 1e9}
         if ms_n < ms_step:
-            # Measured on this pool: the ring wins at N=2 (1 550 vs 1 380 frames/s); from N=4 on rank 0's NVLink ingress is the
-            # bound (2.9 GB per step at N=8) and a layout kernel that stores remotely holds its SMs while the link is busy, whereas
-            # NCCL's copies run beside the next batch's encode (N=8: 2 690 vs 3 490 frames/s).  The headline is the faster delivery
-            # at this N; both are in the line.
+            # Once rank 0's NVLink ingress is the bound (2.9 GB per step at N=8), a layout kernel that stores remotely holds its
+            # SMs while the link is busy, whereas NCCL's copies run beside the next batch's encode, so which delivery is faster
+            # depends on N.  The headline is the faster delivery at this N; both are in the line.
             b = line["nccl_gatherv_baseline"]
             line["ring_delivery"] = {"ms_per_step": ms_step, "fps": fps, "value": line["value"], "nvlink_GBps_into_rank0": line["nvlink_GBps_into_rank0"],
                                      "delivery_share_of_step": line["delivery_share_of_step"]}

@@ -34,13 +34,15 @@ def _tri8(t: torch.Tensor) -> torch.Tensor:
 
 
 def frame(width: int, height: int, index: int = 0, kind: str = "video", alpha: str = "opaque",
-          seed: int = SEED, noise_bits: int = 3, device="cpu") -> torch.Tensor:
-    """(height, width, 4) uint8 RGBA frame number `index`."""
+          seed: int = SEED, noise_bits: int = 3, device="cpu", rows=None) -> torch.Tensor:
+    """(height, width, 4) uint8 RGBA frame number `index`; with rows=(y0, y1) only those rows of it, (y1 - y0, width, 4),
+    bit-identical to the same rows of the whole frame (the int64 intermediates of a whole 16K frame take 8 GiB each)."""
     dev = torch.device(device)
+    y0, y1 = rows if rows is not None else (0, height)
     if kind == "flat":
         px = torch.tensor([0x33, 0x66, 0x99, 0xFF], dtype=torch.uint8, device=dev)
-        return px.expand(height, width, 4).contiguous()
-    y = torch.arange(height, dtype=torch.int64, device=dev).view(height, 1, 1)
+        return px.expand(y1 - y0, width, 4).contiguous()
+    y = torch.arange(y0, y1, dtype=torch.int64, device=dev).view(y1 - y0, 1, 1)
     x = torch.arange(width, dtype=torch.int64, device=dev).view(1, width, 1)
     c = torch.arange(4, dtype=torch.int64, device=dev).view(1, 1, 4)
     lin = (((index * height + y) * width + x) * 4 + c) & _M32
@@ -105,7 +107,7 @@ def _apply_alpha(out, alpha, x, y, width, height):
         r2 = (x - cx) * (x - cx) + (y - cy) * (y - cy)
         rad2 = (min(width, height) // 3) ** 2
         disc = (255 - (255 * r2) // max(rad2, 1)).clamp(0, 255)
-        a = torch.maximum(ramp.expand(height, width, 1), disc)
+        a = torch.maximum(ramp.expand(y.shape[0], width, 1), disc)
         out[..., 3] = a[..., 0].to(torch.uint8)
     else:
         raise ValueError(alpha)

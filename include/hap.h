@@ -4,7 +4,7 @@
  * Drop-in boundary: same six entry points, enum values, callback types and argument meaning as the
  * reference header /root/reference/source/hap.h:40-152 (Vidvox/hap), so a host codec or player that
  * includes the reference's hap.h and links hap.c can link this library instead, unchanged.
- * Behind the boundary the second-stage (Snappy) compression and decompression run as sm_100a CUDA
+ * Behind the boundary the second-stage (Snappy) compression and decompression run as sm_90a CUDA
  * kernels; see include/hap_b200.h for the device-resident batch extensions and INTEGRATION.md for
  * linking.  Every pointer argument may be a host pointer or a CUDA device pointer.
  */

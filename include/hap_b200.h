@@ -2,7 +2,7 @@
  * include/hap_b200.h -- extensions of libhap_b200.so beyond the reference's hap.h.
  *
  * The reference API starts at DXT bytes and moves one frame per call through host memory
- * (/root/reference/source/hap.h:98-137).  A B200 is only busy when whole streams of frames stay in
+ * (Vidvox/hap source/hap.h:98-137).  A GPU is only busy when whole streams of frames stay in
  * HBM, so these entry points add (a) the RGBA side of the path -- the block compressors that sit
  * upstream of HapEncode and the block decoder downstream of HapDecode -- and (b) batched,
  * device-resident, stream-ordered variants.  Plain C ABI: pointers, sizes, no CUDA types (a stream is

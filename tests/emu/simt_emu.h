@@ -5,7 +5,7 @@
 // one after another.  The resume ORDER of fibers is selectable (forward / reverse / seeded random)
 // so that code relying on an accidental thread order between barriers (a missing __syncthreads)
 // fails in at least one mode.  It exists because the build container has no GPU: kernel logic is
-// debugged here against the oracle, then confirmed on the B200 with pytest -m gpu.
+// debugged here against the oracle, then confirmed on the H100 with pytest -m gpu.
 #pragma once
 
 #include <algorithm>

@@ -1,9 +1,9 @@
 #!/usr/bin/env python3
 """TEST INFRASTRUCTURE (it lives under tests/ because it drives the reference build, which only tests may touch).
 How fast do the decode kernels take frames made by the REFERENCE encoder (unmodified hap.c + Google Snappy)?
-bench.py times streams from our own encoder; players mostly meet files written by others.  Run on the GPU box:
+bench.py times streams from our own encoder; players mostly meet files written by others.  Run on a GPU:
 
-    python tests/measure_ref_decode.py [--frames 16] > gpurun_out/ref_decode.json
+    python tests/measure_ref_decode.py [--frames 16] > ref_decode.json
 
 Uses oracle/_ref only to PRODUCE the input frames (on the host, outside every timed region)."""
 import argparse

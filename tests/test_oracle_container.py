@@ -1,5 +1,9 @@
 """Pins the CPU oracle (oracle/hap_oracle.c) against the golden vectors produced by the unmodified
 reference, and differentially against the reference build itself when it is available."""
+import json
+import os
+from base64 import b64decode, b64encode
+
 import numpy as np
 import pytest
 
@@ -91,13 +95,7 @@ def test_oracle_encode_argument_results():
     assert o.encode([p16, p16], [YCOCG, DXT1], [1, 1], [1, 1])[0] == G["ycocg_plus_dxt1"]
 
 
-@pytest.mark.parametrize("seed", range(6))
-def test_oracle_vs_reference_differential(seed):
-    """Random payloads/chunk counts: None frames byte-identical; Snappy frames cross-decode."""
-    ref = oracles.ref_abi()
-    if ref is None:
-        pytest.skip("reference build unavailable")
-    o = oracles.oracle_abi()
+def differential_payload(seed):
     rng = np.random.default_rng(seed)
     blocks = int(rng.integers(1, 600))
     fmt = [DXT1, YCOCG, RGTC1, 0x83F3, 0x8E8C][seed % 5]
@@ -106,15 +104,39 @@ def test_oracle_vs_reference_differential(seed):
     base = rng.integers(0, 256, size=bs * 4, dtype=np.uint8)
     payload = np.tile(base, blocks // 4 + 1)[: blocks * bs].copy()
     payload[:: int(rng.integers(3, 50))] = rng.integers(0, 256)
-    payload = payload.tobytes()
-    k = int(rng.integers(1, 12))
-    assert o.max_encoded_length([len(payload)], [fmt], [k]) == ref.max_encoded_length([len(payload)], [fmt], [k])
+    return payload.tobytes(), fmt, int(rng.integers(1, 12))
+
+
+def reference_answers(ref, seed):
+    """What the reference build returns for seed's payload, in the form tests/golden/ref_differential.json stores."""
+    payload, fmt, k = differential_payload(seed)
     rn, fn = ref.encode([payload], [fmt], [HapCompressorNone], [k])
-    on, fo = o.encode([payload], [fmt], [HapCompressorNone], [k])
-    assert (rn, fn) == (on, fo)
     rs, fs = ref.encode([payload], [fmt], [HapCompressorSnappy], [k])
+    _, fo = oracles.oracle_abi().encode([payload], [fmt], [HapCompressorSnappy], [k])
+    rd, data, dfmt, _ = ref.decode(fo, 0, len(payload))
+    return {"max_len": ref.max_encoded_length([len(payload)], [fmt], [k]), "none": [rn, sha(fn)],
+            "snappy": [rs, b64encode(fs).decode()], "chunk_count": list(ref.chunk_count(fs, 0)),
+            "oracle_snappy_frame": sha(fo), "decode_oracle_frame": [rd, sha(data or b""), dfmt]}
+
+
+@pytest.mark.parametrize("seed", range(6))
+def test_oracle_vs_reference_differential(seed):
+    """Random payloads/chunk counts: None frames byte-identical; Snappy frames cross-decode.  The reference's side comes
+    from tests/golden/ref_differential.json (recorded from the reference build), checked against the build when present."""
+    with open(os.path.join(os.path.dirname(__file__), "golden", "ref_differential.json")) as fh:
+        want = json.load(fh)[str(seed)]
+    ref = oracles.ref_abi()
+    if ref is not None:
+        assert reference_answers(ref, seed) == want
+    o = oracles.oracle_abi()
+    payload, fmt, k = differential_payload(seed)
+    assert o.max_encoded_length([len(payload)], [fmt], [k]) == want["max_len"]
+    on, fo = o.encode([payload], [fmt], [HapCompressorNone], [k])
+    assert [on, sha(fo)] == want["none"]
+    rs, fs = want["snappy"][0], b64decode(want["snappy"][1])
     os_, fo = o.encode([payload], [fmt], [HapCompressorSnappy], [k])
     assert rs == os_ == 0
-    assert ref.chunk_count(fs, 0) == o.chunk_count(fo, 0)
-    assert ref.decode(fo, 0, len(payload))[:3] == (0, payload, fmt)
+    assert list(o.chunk_count(fo, 0)) == want["chunk_count"]
+    # the reference decoded exactly these bytes to the payload
+    assert sha(fo) == want["oracle_snappy_frame"] and want["decode_oracle_frame"] == [0, sha(payload), fmt]
     assert o.decode(fs, 0, len(payload))[:3] == (0, payload, fmt)

@@ -19,3 +19,11 @@ def test_kinds():
     a = synth.frame(64, 64, 0, alpha="ramp")
     assert a[..., 3].min() < 10 and a[..., 3].max() == 255
     assert not torch.equal(synth.frame(64, 64, 0), synth.frame(64, 64, 1))
+
+
+def test_row_bands_equal_the_whole_frame():
+    for kind in ("video", "flat", "noise", "gradient", "texture", "edges"):
+        whole = synth.frame(96, 80, 2, kind=kind, alpha="ramp" if kind != "noise" else "opaque")
+        bands = [synth.frame(96, 80, 2, kind=kind, alpha="ramp" if kind != "noise" else "opaque", rows=(y, min(y + 24, 80)))
+                 for y in range(0, 80, 24)]
+        assert torch.equal(torch.cat(bands), whole), kind

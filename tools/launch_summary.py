@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """ncu launch list (`--metrics gpu__time_duration.sum --csv --log-file x.csv`) -> per-kernel totals and shares, markdown.
-    python tools/launch_summary.py gpurun_out/x_launches.csv [min_ms] > profiles/rNN_launches_summary.md
+    python tools/launch_summary.py validate_out/val_launches.csv [min_ms] > profiles/launches_summary.md
 Only this library's kernels are listed (torch's synthetic-frame kernels are dropped); launches shorter than min_ms
 (default 0: keep all) can be left out, e.g. the empty repair passes of the decoder."""
 import csv

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
-"""Turns an .ncu-rep into the small markdown table kept under profiles/ (run here, no GPU needed):
-    python tools/ncu_summary.py gpurun_out/prof.ncu-rep > profiles/rNN_ncu_<what>.md
+"""Turns an .ncu-rep into a small markdown table (no GPU needed), e.g. under the local, git-ignored profiles/:
+    python tools/ncu_summary.py validate_out/val_prof.ncu-rep > profiles/ncu_<what>.md
 """
 import csv
 import subprocess

@@ -1,6 +1,7 @@
 #!/usr/bin/env python3
-"""DRAM bytes per frame of the main kernels from `ncu --set full` reports -> profiles/traffic.json (read by bench.py for
-roofline.traffic).   python tools/ncu_traffic.py <frames per launch> <report.ncu-rep> [<report> ...]
+"""DRAM bytes per frame of the main kernels from `ncu --set full` reports, as JSON on stdout; saved as profiles/traffic.json
+(local, git-ignored) it is read by bench.py for roofline.traffic.
+    python tools/ncu_traffic.py <frames per launch> <report.ncu-rep> [<report> ...] > profiles/traffic.json
 For every kernel the LARGEST launch of each report is taken (the decode kernels also launch an empty repair pass)."""
 import csv
 import json

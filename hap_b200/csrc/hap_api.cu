@@ -85,6 +85,7 @@ struct DeviceState {
     std::once_flag once;
     bool ready = false;
     int sm_count = 132;
+    int k5_ctas_per_sm = 1;   // resident CTAs of the fragment compressor per SM (its persistent grid is this x sm_count)
 };
 DeviceState g_dev[kMaxDevices];
 std::atomic<int> g_default_device{-1};
@@ -105,7 +106,10 @@ void device_init(int dev)
     ok = ok && cudaFuncSetAttribute(snappy_index_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IndexSmem)) == cudaSuccess;
     ok = ok && cudaFuncSetAttribute(snappy_encode_fragments_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                     (int)sizeof(EncodeSmem)) == cudaSuccess;
+    ok = ok && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&d.k5_ctas_per_sm, snappy_encode_fragments_kernel, kEncThreads,
+                                                             sizeof(EncodeSmem)) == cudaSuccess;
     if (!ok) { cudaGetLastError(); return; }
+    if (d.k5_ctas_per_sm < 1) d.k5_ctas_per_sm = 1;
     d.ready = true;
 }
 
@@ -297,8 +301,9 @@ uint32_t launch_encode(const uint8_t *base, const FrameGeom &G, uint32_t frames,
 #ifndef HAPB200_ENC_PERSISTENT
 #define HAPB200_ENC_PERSISTENT 1
 #endif
-    // one resident CTA per SM strides over the fragments (the kernel's 131 KB of shared memory allow no second one)
-    const unsigned k5_grid = HAPB200_ENC_PERSISTENT ? (unsigned)(nfrag < (uint64_t)sm_count() ? nfrag : (uint64_t)sm_count()) : (unsigned)nfrag;
+    // every CTA that can be resident at once (two per SM with the kernel's 108 KB of shared memory) strides over the fragments
+    const uint64_t k5_resident = (uint64_t)sm_count() * (uint64_t)g_dev[t_device].k5_ctas_per_sm;
+    const unsigned k5_grid = HAPB200_ENC_PERSISTENT ? (unsigned)(nfrag < k5_resident ? nfrag : k5_resident) : (unsigned)nfrag;
     HAP_KLAUNCH(kStSnappyEncode, snappy_encode_fragments_kernel, dim3(k5_grid), dim3(kEncThreads), sizeof(EncodeSmem), st, base, G,
                 (uint32_t)nfrag, scratch.as<uint8_t>(), fsize.as<uint32_t>(), write_index ? fent.as<uint8_t>() : (uint8_t *)nullptr);
     HAP_KLAUNCH(kStPlan, hap_plan_frames_kernel, dim3(frames), dim3(kPlanThreads), 0, st, G, base, fsize.as<uint32_t>(),

@@ -4,8 +4,8 @@
 // (/root/reference/source/hap.c:448-476, call site :453).  The reference's loop is serial over chunks
 // and Snappy is serial inside a chunk; here a chunk is cut into independent 32 KiB FRAGMENTS (a raw
 // Snappy stream is varint(length) followed by elements, so fragment element streams concatenate
-// into one legal chunk stream as long as copies never reach outside their fragment), one resident CTA
-// per SM striding over the fragments, and inside a fragment every 8-byte unit is handled on its own:
+// into one legal chunk stream as long as copies never reach outside their fragment), a persistent grid
+// of CTAs (two per SM) striding over the fragments, and inside a fragment every 8-byte unit is handled on its own:
 //   1. first-occurrence hash of every aligned word (shared-memory table, atomicMin => deterministic);
 //   2. each word picks a source: the word one DXT block back when its whole block repeats the
 //      previous block (block RLE, decodes as one periodic fill), else the first earlier occurrence
@@ -23,7 +23,7 @@
 
 namespace hapb200 {
 
-constexpr int kEncThreads = 1024;
+constexpr int kEncThreads = 512;        // two CTAs per SM: 2 x 512 threads x 64 registers fill the register file
 constexpr int kEncWarps = kEncThreads / 32;
 constexpr int kFragBytes = 32768;
 constexpr int kFragCap = kFragBytes + 32;   // element stream of a fragment never exceeds n + 3
@@ -34,51 +34,50 @@ constexpr int kFragEntryStride = 272;             // bytes reserved per fragment
 static_assert(kFragEntryPieces <= kFragEntryStride, "entries of one fragment fit their scratch slot");
 
 // Shared memory of one fragment.  The unit of every decision is 8 BYTES (a DXT1 / RGTC1 block, half a DXT5 block): thread t
-// owns the 4 consecutive units [4t, 4t+4) and keeps them (and every per-unit quantity) in registers; shared memory only
+// owns the 8 consecutive units [8t, 8t+8) and keeps them (and every per-unit quantity) in registers; shared memory only
 // carries what OTHER threads read: the data (random match verification), the hash table, the strip-boundary values of the
 // per-unit arrays, and -- for the last step, which re-distributes the units over the threads -- positions, run starts and
 // distances.  (Round 1 decided per 4-byte word: twice the elements in every step, and 4-byte matches that were demoted
 // again because a copy element costs 3 bytes.  Matches that start at an odd word are lost; DXT payloads hardly have any.)
-#ifndef HAPB200_K5_ROUNDS
-#define HAPB200_K5_ROUNDS 1
-#endif
 constexpr int kFragUnits = kFragBytes / 8;        // 4096
-constexpr int kUnitStrip = kFragUnits / kEncThreads;   // 4 units per thread
-static_assert(kUnitStrip == 4, "the strip code below moves 4 uint16 values per thread as one 8-byte access");
+constexpr int kUnitStrip = kFragUnits / kEncThreads;   // 8 units per thread
+static_assert(kUnitStrip == 8, "the strip code below moves 8 uint16 values per thread as one 16-byte access");
 struct EncodeSmem {
     uint2 data[kFragUnits + 2];                     // input units
     union {
         uint32_t table[1 << kEncHashBits];          // first occurrence of every hashed unit
         struct {
-            uint16_t a[kFragUnits];                 // final distance per unit (read by the re-dealt output step)
+            uint16_t a[kFragUnits];                 // final distance per unit (written by the propagation once the table is dead)
             uint16_t b[kFragUnits];                 // run start per unit
             uint16_t c[kFragUnits];                 // stream position per unit
         } h;
     } u;
-    uint16_t da[kFragUnits];                        // candidate distances (ping) | one of the two holds the final distances,
-    uint16_t db[kFragUnits];                        // candidate distances (pong) | the other then the run ends (stored at the run start)
+    uint16_t da[kFragUnits];                        // candidate distances, then the run ends (stored at the run start)
     uint32_t warp_tot[kEncWarps];
     uint32_t entry[kFragEntryStride];               // fragment index: offset of the first element start in every 128 bytes of the stream
     uint32_t total;
     alignas(16) uint32_t out[(kFragCap + 3) / 4 + 6];   // the element stream (copied out in 16-byte words)
 };
+// Two CTAs per SM: an H100 SM has 228 KiB of shared memory for CTAs and reserves 1 KiB of it per CTA, so each of two CTAs
+// may use (233,472 - 2 x 1,024) / 2 = 115,712 bytes.
+static_assert(sizeof(EncodeSmem) <= 115712, "two encode CTAs fit the shared memory of one SM");
 
 __device__ __forceinline__ uint32_t enc_hash(uint2 u) { return ((u.x * 0x9E3779B1u) ^ (u.y * 0x85EBCA6Bu)) >> (32 - kEncHashBits); }
 __device__ __forceinline__ bool same_unit(uint2 a, uint2 b) { return a.x == b.x && a.y == b.y; }
 
 __device__ __forceinline__ uint32_t literal_header_bytes(uint32_t len) { return len <= 60 ? 1u : len <= 256 ? 2u : 3u; }
 
-__device__ __forceinline__ void store_strip16(uint16_t *arr, uint32_t base, const uint32_t v[4])
+__device__ __forceinline__ void store_strip16(uint16_t *arr, uint32_t base, const uint32_t v[kUnitStrip])
 {
-    *reinterpret_cast<uint2 *>(arr + base) = make_uint2(v[0] | (v[1] << 16), v[2] | (v[3] << 16));
+    *reinterpret_cast<uint4 *>(arr + base) = make_uint4(v[0] | (v[1] << 16), v[2] | (v[3] << 16), v[4] | (v[5] << 16), v[6] | (v[7] << 16));
 }
 
 // Inclusive max / sum over the block of one value per thread; returns the exclusive prefix for this thread and
-// the block total.  Two barriers.  The 32 warp totals are scanned by every warp with shuffles (lane w holds the
-// total of warp w) instead of a 32-step loop over shared memory.
+// the block total.  Two barriers.  The warp totals are scanned by every warp with shuffles (lane w holds the
+// total of warp w; lanes past the last warp hold the identity, 0 for both) instead of a loop over shared memory.
 __device__ __forceinline__ uint32_t enc_block_excl(uint32_t v, bool is_max, uint32_t *total, uint32_t *warp_tot)
 {
-    static_assert(kEncWarps == 32, "one warp total per lane");
+    static_assert(kEncWarps <= 32, "one warp total per lane");
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     uint32_t incl = v;
 #pragma unroll
@@ -90,7 +89,7 @@ __device__ __forceinline__ uint32_t enc_block_excl(uint32_t v, bool is_max, uint
     if (lane == 0) prev = 0;
     if (lane == 31) warp_tot[warp] = incl;
     __syncthreads();
-    uint32_t wi = warp_tot[lane];
+    uint32_t wi = lane < kEncWarps ? warp_tot[lane] : 0u;
 #pragma unroll
     for (int d = 1; d < 32; d <<= 1) {
         uint32_t o = __shfl_up_sync(HAP_FULL_MASK, wi, d);
@@ -104,30 +103,40 @@ __device__ __forceinline__ uint32_t enc_block_excl(uint32_t v, bool is_max, uint
     return is_max ? (base > prev ? base : prev) : base + prev;
 }
 
-// One fragment: U units (8 bytes each; U <= kFragUnits) already in S.data AND in the caller's registers d[4] (units
-// 4t..4t+3) -> element stream written to S.out as bytes; returns its size (all threads).
+// One fragment: U units (8 bytes each; U <= kFragUnits) already in S.data AND in the caller's registers d[8] (units
+// 8t..8t+7) -> element stream written to S.out as bytes; returns its size (all threads).
 // period_units = DXT block size in units (1 or 2).
 // FULL = the fragment has all kFragUnits units (31 of 32 fragments of a 1 MiB chunk): every per-unit bounds test
 // folds away at compile time.
 template <bool FULL>
-__device__ __forceinline__ uint32_t compress_fragment(EncodeSmem &S, const uint2 d[4], uint32_t Udyn, uint32_t period_units)
+__device__ __forceinline__ uint32_t compress_fragment(EncodeSmem &S, const uint2 d[kUnitStrip], uint32_t Udyn, uint32_t period_units)
 {
     const uint32_t t = threadIdx.x;
     const uint32_t U = FULL ? (uint32_t)kFragUnits : Udyn;
     const uint32_t i0 = t * kUnitStrip;              // first unit of my strip
     const uint32_t nv = FULL ? (uint32_t)kUnitStrip : (i0 >= U ? 0u : (U - i0 < (uint32_t)kUnitStrip ? U - i0 : (uint32_t)kUnitStrip));  // my valid units
 
-    // 1. first occurrence of every unit (the table was initialised by the caller, before the barrier)
-    uint32_t hsh[4];
+    // 1. first occurrence of every unit (the table was initialised by the caller, before the barrier).  A unit whose hash
+    //    equals that of one of the two units before it leaves the atomicMin to that lower unit: the table ends the same,
+    //    and on flat content (letterbox bars, repeated blocks) a warp no longer sends 32 lanes to one address.
+    uint32_t hsh[kUnitStrip];
 #pragma unroll
-    for (int k = 0; k < kUnitStrip; k++) {
-        hsh[k] = enc_hash(d[k]);
-        if ((uint32_t)k < nv) atomicMin(&S.u.table[hsh[k]], i0 + k);
+    for (int k = 0; k < kUnitStrip; k++) hsh[k] = enc_hash(d[k]);
+    {
+        const uint32_t lane = t & 31;
+        const uint32_t p1 = __shfl_up_sync(HAP_FULL_MASK, hsh[kUnitStrip - 1], 1), p2 = __shfl_up_sync(HAP_FULL_MASK, hsh[kUnitStrip - 2], 1);
+#pragma unroll
+        for (int k = 0; k < kUnitStrip; k++) {
+            const bool has1 = k >= 1 || lane > 0, has2 = k >= 2 || lane > 0;
+            const uint32_t h1 = k >= 1 ? hsh[k - 1] : p1, h2 = k >= 2 ? hsh[k - 2] : k == 1 ? p1 : p2;
+            const bool dup = (has1 && h1 == hsh[k]) || (has2 && h2 == hsh[k]);
+            if ((uint32_t)k < nv && !dup) atomicMin(&S.u.table[hsh[k]], i0 + k);
+        }
     }
     __syncthreads();
 
     // 2. candidate distance per unit: first earlier occurrence, or one block back when the whole block repeats
-    uint32_t dd[4];
+    uint32_t dd[kUnitStrip];
 #pragma unroll
     for (int k = 0; k < kUnitStrip; k++) {
         dd[k] = 0;
@@ -137,10 +146,12 @@ __device__ __forceinline__ uint32_t compress_fragment(EncodeSmem &S, const uint2
         }
     }
     if (period_units == 2) {
-        // DXT5-sized blocks: units (2b, 2b+1); the block repeats when both units equal the block before
+        // DXT5-sized blocks: units (2b, 2b+1); the block repeats when both of its units exist and equal the block before
         const uint2 p0 = i0 >= 2 ? S.data[i0 - 2] : make_uint2(0, 0), p1 = i0 >= 2 ? S.data[i0 - 1] : make_uint2(0, 0);
         if (i0 >= 2 && nv >= 2 && same_unit(p0, d[0]) && same_unit(p1, d[1])) { dd[0] = 2; dd[1] = 2; }
-        if (nv >= 4 && same_unit(d[0], d[2]) && same_unit(d[1], d[3])) { dd[2] = 2; dd[3] = 2; }
+#pragma unroll
+        for (int k = 2; k < kUnitStrip; k += 2)
+            if ((uint32_t)k + 2 <= nv && same_unit(d[k - 2], d[k]) && same_unit(d[k - 1], d[k + 1])) { dd[k] = 2; dd[k + 1] = 2; }
     } else {
         const uint2 p = i0 >= 1 ? S.data[i0 - 1] : make_uint2(0, 0);
         if (i0 >= 1 && nv >= 1 && same_unit(p, d[0])) dd[0] = 1;
@@ -151,49 +162,43 @@ __device__ __forceinline__ uint32_t compress_fragment(EncodeSmem &S, const uint2
     store_strip16(S.da, i0, dd);
     __syncthreads();
 
-    // 2b. propagation (two rounds): a unit that is not yet part of a run adopts its left (else right) neighbour's
+    // 2b. propagation (one round): a unit that is not yet part of a run adopts its left (else right) neighbour's
     //     distance when its own data also matches there.  First occurrences of neighbouring units often point at
     //     different earlier blocks; this re-aligns them and recovers most of what a greedy match extension finds.
-    uint16_t *cur = S.da, *nxt = S.db;
+    //     Every unit decides from the distances before the round (S.da), so the result does not depend on the order
+    //     in which threads run.  (Measured on the emulator cases: with 8-byte units ONE round recovers what two did --
+    //     frame sizes equal on picture content, +0.1 .. 0.5 % on the stitched random cases; none costs 5 .. 16 %.)
     {
-#pragma unroll 1
-        for (int round = 0; round < HAPB200_K5_ROUNDS; round++) {
-            const uint32_t lb = i0 > 0 ? cur[i0 - 1] : 0u;
-            const uint32_t rb = i0 + kUnitStrip < U ? cur[i0 + kUnitStrip] : 0u;
-            uint32_t nd[4];
+        const uint32_t lb = i0 > 0 ? S.da[i0 - 1] : 0u;
+        const uint32_t rb = i0 + kUnitStrip < U ? S.da[i0 + kUnitStrip] : 0u;
+        uint32_t l = lb;   // the left neighbour's distance before the round
 #pragma unroll
-            for (int k = 0; k < kUnitStrip; k++) {
-                const uint32_t l = k > 0 ? dd[k - 1] : lb, r = k < kUnitStrip - 1 ? dd[k + 1] : rb;
-                const uint32_t cd = dd[k], i = i0 + k;
-                nd[k] = cd;
-                if ((uint32_t)k < nv && !(cd != 0 && (cd == l || cd == r))) {
-                    // one look-up decides: the left neighbour's distance if there is one, else the right one's
-                    const uint32_t cand = l != 0 ? l : r;
-                    if (cand != 0 && i >= cand && same_unit(S.data[i - cand], d[k])) nd[k] = cand;
-                    else if (l != 0 && r != 0 && r != l && i >= r && same_unit(S.data[i - r], d[k])) nd[k] = r;
-                }
+        for (int k = 0; k < kUnitStrip; k++) {
+            const uint32_t r = k < kUnitStrip - 1 ? dd[k + 1] : rb;
+            const uint32_t cd = dd[k], i = i0 + k;
+            if ((uint32_t)k < nv && !(cd != 0 && (cd == l || cd == r))) {
+                // one look-up decides: the left neighbour's distance if there is one, else the right one's
+                const uint32_t cand = l != 0 ? l : r;
+                if (cand != 0 && i >= cand && same_unit(S.data[i - cand], d[k])) dd[k] = cand;
+                else if (l != 0 && r != 0 && r != l && i >= r && same_unit(S.data[i - r], d[k])) dd[k] = r;
             }
-#pragma unroll
-            for (int k = 0; k < kUnitStrip; k++) dd[k] = nd[k];
-            store_strip16(nxt, i0, dd);
-            __syncthreads();
-            uint16_t *tmp = cur; cur = nxt; nxt = tmp;
+            l = cd;
         }
     }
-    // `cur` holds the final distances (read across strip boundaries below); the other buffer is free: it takes the run ends.
-    // (Measured on the emulator cases: with 8-byte units ONE round recovers what two did -- frame sizes equal on picture
-    // content, +0.1 .. 0.5 % on the stitched random cases; none costs 5 .. 16 %.)
-    const uint16_t *fin = cur;
-    uint16_t *ends = nxt;
-    // (a single matching unit is kept: an 8-byte copy costs 3 bytes)
-    store_strip16(S.u.h.a, i0, dd);   // the hash table is dead: its space holds the final distances
+    // The hash table is dead since the barrier above: its space takes the final distances (read across strip boundaries
+    // below and by the re-dealt output step); S.da is free once every thread has read its neighbours there, and takes
+    // the run ends.  (A single matching unit is kept: an 8-byte copy costs 3 bytes.)
+    store_strip16(S.u.h.a, i0, dd);
+    __syncthreads();
+    const uint16_t *fin = S.u.h.a;
+    uint16_t *ends = S.da;
 
     // 3. run start of every unit (max-scan of "i+1 where a run starts") and run ends (stored at the run start)
-    uint32_t rs[4];
+    uint32_t rs[kUnitStrip];
     {
         const uint32_t lb = i0 > 0 ? fin[i0 - 1] : 0u;
         uint32_t last = 0;  // (index + 1) of the last run start inside my strip so far
-        uint32_t loc[4];
+        uint32_t loc[kUnitStrip];
 #pragma unroll
         for (int k = 0; k < kUnitStrip; k++) {
             const uint32_t prev = k > 0 ? dd[k - 1] : lb;
@@ -214,7 +219,7 @@ __device__ __forceinline__ uint32_t compress_fragment(EncodeSmem &S, const uint2
     __syncthreads();
 
     // 4. bytes each unit contributes and their exclusive prefix sum
-    uint32_t pos[4];
+    uint32_t pos[kUnitStrip];
     {
         uint32_t run = 0;
 #pragma unroll
@@ -239,8 +244,8 @@ __device__ __forceinline__ uint32_t compress_fragment(EncodeSmem &S, const uint2
         if (t == 0) S.total = tot;
     }
 
-    // 5. every unit writes its own bytes.  Ownership changes for this step: thread t takes units t, t + 1024, ... so that
-    //    the lanes of a warp write neighbouring bytes of the stream (with the strip layout they sit 32 bytes apart: bank
+    // 5. every unit writes its own bytes.  Ownership changes for this step: thread t takes units t, t + 512, ... so that
+    //    the lanes of a warp write neighbouring bytes of the stream (with the strip layout they sit 64 bytes apart: bank
     //    conflicts on every store).  Positions, run starts and distances travel through shared memory as 16-bit strips.
     //    Inside a literal run the stream is the input shifted by (p & 3) bytes, so a unit writes TWO aligned 32-bit words
     //    made of its own bytes and the next unit's first bytes; only the two ends of a run, headers and copy elements are
@@ -366,13 +371,17 @@ __device__ __forceinline__ FragRef locate_fragment(const uint8_t *dxt, const Fra
     return r;
 }
 
-// A thread's 4 units of a fragment, from global memory: two 16-byte loads when possible
-__device__ __forceinline__ void load_strip(const FragRef &fr, uint32_t i0, uint2 d[4])
+// A thread's 8 units of a fragment, from global memory: four 16-byte loads when possible
+__device__ __forceinline__ void load_strip(const FragRef &fr, uint32_t i0, uint2 d[kUnitStrip])
 {
     if ((((uintptr_t)fr.in) & 15) == 0 && i0 + kUnitStrip <= fr.units) {
         const uint4 *in4 = reinterpret_cast<const uint4 *>(fr.in) + (i0 >> 1);
-        const uint4 a = in4[0], b = in4[1];
-        d[0] = make_uint2(a.x, a.y); d[1] = make_uint2(a.z, a.w); d[2] = make_uint2(b.x, b.y); d[3] = make_uint2(b.z, b.w);
+#pragma unroll
+        for (int k = 0; k < kUnitStrip / 2; k++) {
+            const uint4 a = in4[k];
+            d[2 * k] = make_uint2(a.x, a.y);
+            d[2 * k + 1] = make_uint2(a.z, a.w);
+        }
     } else {
 #pragma unroll
         for (int k = 0; k < kUnitStrip; k++) {
@@ -387,13 +396,12 @@ __device__ __forceinline__ void load_strip(const FragRef &fr, uint32_t i0, uint2
     }
 }
 
-// A fixed grid (one CTA per SM: the kernel needs 123 KB of shared memory) strides over the nfrag = frames *
-// frags_per_frame fragments of the batch.  A thread's units of the NEXT fragment are loaded before the current one is
-// compressed, so the HBM latency of the input and the turn-over between CTAs -- both fully exposed with a single CTA
-// per SM -- are covered by a fragment's worth of work.
+// A persistent grid (as many CTAs as fit on the device at once: two per SM, the kernel needs 108 KB of shared memory)
+// strides over the nfrag = frames * frags_per_frame fragments of the batch.  While one CTA of an SM waits at a barrier
+// or for the HBM latency of its next fragment's input, the other one computes.
 // dxt: base pointer of the texture bytes; scratch: [nfrag][kFragCap]; frag_size: [nfrag] (kFragStoredRaw when the
 // fragment was not compressed); frag_entries: [nfrag][kFragEntryStride] or nullptr (fragment index, hap_index.h).
-__global__ void __launch_bounds__(kEncThreads) snappy_encode_fragments_kernel(
+__global__ void __launch_bounds__(kEncThreads, 2) snappy_encode_fragments_kernel(
     const uint8_t *__restrict__ dxt, FrameGeom G, uint32_t nfrag, uint8_t *__restrict__ scratch, uint32_t *__restrict__ frag_size,
     uint8_t *__restrict__ frag_entries)
 {
@@ -401,49 +409,34 @@ __global__ void __launch_bounds__(kEncThreads) snappy_encode_fragments_kernel(
     EncodeSmem &S = *reinterpret_cast<EncodeSmem *>(smem_raw);
     const int t = threadIdx.x;
     const uint32_t i0 = (uint32_t)t * kUnitStrip;
-    uint32_t gfrag = blockIdx.x;
-    if (gfrag >= nfrag) return;
-    FragRef cur = locate_fragment(dxt, G, gfrag);
-    uint2 d[4];
-    load_strip(cur, i0, d);
-    for (;;) {
-        const uint32_t next = gfrag + gridDim.x;
-        FragRef nxt;
-        uint2 nd[4];
-        const bool more = next < nfrag;
-        if (more) {
-            nxt = locate_fragment(dxt, G, next);
-            load_strip(nxt, i0, nd);     // in flight while this fragment is compressed
-        }
+    for (uint32_t gfrag = blockIdx.x; gfrag < nfrag; gfrag += gridDim.x) {
+        const FragRef cur = locate_fragment(dxt, G, gfrag);
         if (cur.units == 0) {
             if (t == 0) frag_size[gfrag] = kFragStoredRaw;
-        } else {
-            const uint32_t U = cur.units;
-            *reinterpret_cast<uint4 *>(&S.data[i0]) = make_uint4(d[0].x, d[0].y, d[1].x, d[1].y);
-            *reinterpret_cast<uint4 *>(&S.data[i0 + 2]) = make_uint4(d[2].x, d[2].y, d[3].x, d[3].y);
-            {
-                uint4 *tb = reinterpret_cast<uint4 *>(S.u.table);
-                const uint4 ones = make_uint4(0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu);
-                for (int q = t; q < (1 << kEncHashBits) / 4; q += kEncThreads) tb[q] = ones;
-                if (t < kFragEntryStride) S.entry[t] = kIndexNoEntry;
-            }
-            __syncthreads();
-            const uint32_t period_units = (cur.second ? G.s[1].period_words : G.s[0].period_words) >> 1;   // 8-byte blocks: 1, 16-byte blocks: 2
-            const uint32_t total = U == (uint32_t)kFragUnits ? compress_fragment<true>(S, d, U, period_units)
-                                                             : compress_fragment<false>(S, d, U, period_units);
-            uint8_t *o = scratch + (uint64_t)gfrag * kFragCap;
-            const uint4 *o4s = reinterpret_cast<const uint4 *>(S.out);
-            uint4 *o4 = reinterpret_cast<uint4 *>(o);       // (scratch slots are kFragCap = 32800 bytes apart: 16-byte aligned)
-            for (uint32_t i = t; i < (total + 15) / 16; i += kEncThreads) o4[i] = o4s[i];
-            if (frag_entries != nullptr && t < kFragEntryStride) frag_entries[(uint64_t)gfrag * kFragEntryStride + t] = (uint8_t)S.entry[t];
-            if (t == 0) frag_size[gfrag] = total;
-            __syncthreads();   // S.out, S.data and the tables are rewritten by the next fragment
+            continue;
         }
-        if (!more) break;
-        gfrag = next;
-        cur = nxt;
+        const uint32_t U = cur.units;
+        uint2 d[kUnitStrip];
+        load_strip(cur, i0, d);
 #pragma unroll
-        for (int k = 0; k < kUnitStrip; k++) d[k] = nd[k];
+        for (int k = 0; k < kUnitStrip; k += 2) *reinterpret_cast<uint4 *>(&S.data[i0 + k]) = make_uint4(d[k].x, d[k].y, d[k + 1].x, d[k + 1].y);
+        {
+            uint4 *tb = reinterpret_cast<uint4 *>(S.u.table);
+            const uint4 ones = make_uint4(0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu);
+            for (int q = t; q < (1 << kEncHashBits) / 4; q += kEncThreads) tb[q] = ones;
+            if (t < kFragEntryStride) S.entry[t] = kIndexNoEntry;
+        }
+        __syncthreads();
+        const uint32_t period_units = (cur.second ? G.s[1].period_words : G.s[0].period_words) >> 1;   // 8-byte blocks: 1, 16-byte blocks: 2
+        const uint32_t total = U == (uint32_t)kFragUnits ? compress_fragment<true>(S, d, U, period_units)
+                                                         : compress_fragment<false>(S, d, U, period_units);
+        uint8_t *o = scratch + (uint64_t)gfrag * kFragCap;
+        const uint4 *o4s = reinterpret_cast<const uint4 *>(S.out);
+        uint4 *o4 = reinterpret_cast<uint4 *>(o);       // (scratch slots are kFragCap = 32800 bytes apart: 16-byte aligned)
+        for (uint32_t i = t; i < (total + 15) / 16; i += kEncThreads) o4[i] = o4s[i];
+        if (frag_entries != nullptr && t < kFragEntryStride) frag_entries[(uint64_t)gfrag * kFragEntryStride + t] = (uint8_t)S.entry[t];
+        if (t == 0) frag_size[gfrag] = total;
+        __syncthreads();   // S.out, S.data and the tables are rewritten by the next fragment
     }
 }
 

@@ -119,37 +119,41 @@ int pointer_device(const void *p)   // device ordinal of a device / managed poin
     if (!p || cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return -1; }
     return (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged) ? a.device : -1;
 }
+inline bool is_device(const void *p) { return pointer_device(p) >= 0; }
 
-// One per entry point.  `hints`: the call's buffers; the first device pointer among them decides the device.
+// The device of a codec call.  `hints`: the call's buffers; the first device pointer among them decides the device,
+// else the process default.  -1 when there is none.
+int call_device(std::initializer_list<const void *> hints)
+{
+    static std::once_flag env_once;
+    std::call_once(env_once, [] {
+        // process-wide defaults of the options (HapB200SetOption overrides them)
+        if (const char *e = getenv("HAPB200_WRITE_INDEX")) g_write_index.store(atoi(e) != 0);
+        if (const char *e = getenv("HAPB200_USE_INDEX")) g_use_index.store(atoi(e) != 0);
+        if (const char *e = getenv("HAPB200_WRITE_OFFSET_TABLE")) g_write_offsets.store(atoi(e) != 0);
+        if (const char *e = getenv("HAPB200_CHROMA_REFINE")) g_chroma_refine.store(atoi(e) != 0);
+    });
+    for (const void *h : hints)
+        if (const int d = pointer_device(h); d >= 0) return d;
+    int cur = -1;
+    if (cudaGetDevice(&cur) != cudaSuccess) { cudaGetLastError(); return -1; }
+    int expected = -1;
+    g_default_device.compare_exchange_strong(expected, cur);   // first call: this thread's device becomes the default
+    return g_default_device.load();
+}
+
+// One per entry point: runs the call on `device` (set up on its first use) and restores the caller's device.
 struct DeviceGuard {
     int saved = -1;
     bool ok = false;
-    DeviceGuard(std::initializer_list<const void *> hints)
+    explicit DeviceGuard(int device)
     {
-        static std::once_flag env_once;
-        std::call_once(env_once, [] {
-            // process-wide defaults of the two options (HapB200SetOption overrides them)
-            if (const char *e = getenv("HAPB200_WRITE_INDEX")) g_write_index.store(atoi(e) != 0);
-            if (const char *e = getenv("HAPB200_USE_INDEX")) g_use_index.store(atoi(e) != 0);
-            if (const char *e = getenv("HAPB200_WRITE_OFFSET_TABLE")) g_write_offsets.store(atoi(e) != 0);
-            if (const char *e = getenv("HAPB200_CHROMA_REFINE")) g_chroma_refine.store(atoi(e) != 0);
-        });
         if (cudaGetDevice(&saved) != cudaSuccess) { cudaGetLastError(); saved = -1; return; }
-        int want = -1;
-        for (const void *h : hints) {
-            want = pointer_device(h);
-            if (want >= 0) break;
-        }
-        if (want < 0) {
-            int expected = -1;
-            g_default_device.compare_exchange_strong(expected, saved);   // first call: this thread's device becomes the default
-            want = g_default_device.load();
-        }
-        if (want < 0 || want >= kMaxDevices) return;
-        if (want != saved && cudaSetDevice(want) != cudaSuccess) { cudaGetLastError(); return; }
-        std::call_once(g_dev[want].once, device_init, want);
-        t_device = want;
-        ok = g_dev[want].ready;
+        if (device < 0 || device >= kMaxDevices) return;
+        if (device != saved && cudaSetDevice(device) != cudaSuccess) { cudaGetLastError(); return; }
+        std::call_once(g_dev[device].once, device_init, device);
+        t_device = device;
+        ok = g_dev[device].ready;
     }
     ~DeviceGuard()
     {
@@ -158,8 +162,8 @@ struct DeviceGuard {
         cudaGetLastError();
     }
 };
-#define HAP_ENTER(...)                                     \
-    DeviceGuard hap_device_guard_({__VA_ARGS__});          \
+#define HAP_ENTER(...)                                           \
+    DeviceGuard hap_device_guard_(call_device({__VA_ARGS__}));   \
     if (!hap_device_guard_.ok) return HapResult_Internal_Error
 
 inline int sm_count() { return g_dev[t_device].sm_count; }
@@ -189,10 +193,8 @@ struct CallStream {
     std::unique_lock<std::mutex> serial;
     static std::mutex &pool_mu() { static std::mutex m; return m; }
     static std::vector<PooledStream> &pool() { static std::vector<PooledStream> v[kMaxDevices]; return v[t_device]; }
-    int device = 0;
     explicit CallStream(bool all_host)
     {
-        device = t_device;
         if (all_host) {
             {
                 std::lock_guard<std::mutex> l(pool_mu());
@@ -231,18 +233,10 @@ struct CallStream {
         if (pooled) {
             g_call_mem = nullptr;
             std::lock_guard<std::mutex> l(pool_mu());
-            static_cast<void>(device);
             pool().push_back(ps);   // (t_device is still this call's device: the guard outlives the stream)
         }
     }
 };
-
-bool is_device_pointer(const void *p)
-{
-    cudaPointerAttributes a;
-    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
-    return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
-}
 
 // stream-ordered scratch
 struct DevBuf {
@@ -280,6 +274,31 @@ bool codec_info(unsigned codec, CodecInfo &c)
     }
 }
 
+// hap.c:551-559 (SURVEY.md Q5): of two textures, one must be scaled YCoCg DXT5 or alpha RGTC1
+bool texture_formats_ok(unsigned count, const unsigned *f)
+{
+    return count != 2 || f[0] == HapFmt_YCoCg_DXT5 || f[1] == HapFmt_YCoCg_DXT5 || f[0] == HapFmt_A_RGTC1 || f[1] == HapFmt_A_RGTC1;
+}
+
+// width x height RGBA pictures, rows rowBytes apart.  aligned: the batch entry points' rules besides (16-byte aligned rows,
+// picture address and picture stride).
+bool rgba_geometry_ok(const void *rgba, unsigned width, unsigned height, unsigned long rowBytes, unsigned long frameStride, bool aligned)
+{
+    if (!rgba || width == 0 || height == 0 || width % 4 || height % 4 || rowBytes < 4ul * width) return false;
+    return !aligned || (rowBytes % 16 == 0 && ((uintptr_t)rgba | frameStride) % 16 == 0);
+}
+
+// The batch entry points run `work` on the caller's stream, or on the legacy stream when the caller gave none; then they
+// return only once the work is done.
+template <class Work>
+uint32_t on_batch_stream(void *stream, Work &&work)
+{
+    const cudaStream_t st = stream ? (cudaStream_t)stream : kLegacyStream;
+    uint32_t r = work(st);
+    if (r == HapResult_No_Error && !stream && cudaStreamSynchronize(st) != cudaSuccess) { cudaGetLastError(); r = HapResult_Internal_Error; }
+    return r;
+}
+
 // ---- device pipelines (all asynchronous on `st`) -------------------------------------------------
 
 // textures of `frames` frames (device, described by G.s[i].in_offset/in_stride relative to `base`) ->
@@ -298,12 +317,9 @@ uint32_t launch_encode(const uint8_t *base, const FrameGeom &G, uint32_t frames,
         cudaGetLastError();
         return HapResult_Internal_Error;
     }
-#ifndef HAPB200_ENC_PERSISTENT
-#define HAPB200_ENC_PERSISTENT 1
-#endif
     // every CTA that can be resident at once (two per SM with the kernel's 108 KB of shared memory) strides over the fragments
     const uint64_t k5_resident = (uint64_t)sm_count() * (uint64_t)g_dev[t_device].k5_ctas_per_sm;
-    const unsigned k5_grid = HAPB200_ENC_PERSISTENT ? (unsigned)(nfrag < k5_resident ? nfrag : k5_resident) : (unsigned)nfrag;
+    const unsigned k5_grid = (unsigned)(nfrag < k5_resident ? nfrag : k5_resident);
     HAP_KLAUNCH(kStSnappyEncode, snappy_encode_fragments_kernel, dim3(k5_grid), dim3(kEncThreads), sizeof(EncodeSmem), st, base, G,
                 (uint32_t)nfrag, scratch.as<uint8_t>(), fsize.as<uint32_t>(), write_index ? fent.as<uint8_t>() : (uint8_t *)nullptr);
     HAP_KLAUNCH(kStPlan, hap_plan_frames_kernel, dim3(frames), dim3(kPlanThreads), 0, st, G, base, fsize.as<uint32_t>(),
@@ -313,6 +329,15 @@ uint32_t launch_encode(const uint8_t *base, const FrameGeom &G, uint32_t frames,
                 scratch.as<uint8_t>(), fsize.as<uint32_t>(), fdst.as<uint32_t>(), fidx.as<uint32_t>(),
                 write_index ? fent.as<uint8_t>() : (const uint8_t *)nullptr, out, out_stride);
     return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
+}
+
+// the scaled-YCoCg kinds have a chroma-refining variant (HAPB200_OPTION_CHROMA_REFINE)
+template <int KIND>
+void launch_bc_encode(dim3 grid, cudaStream_t st, const uint8_t *rgba, const BcGeom &g, uint8_t *blocks, bool refine)
+{
+    constexpr bool kRefines = KIND == kBcYCoCg || KIND == kBcYCoCgPlusAlpha;
+    if (kRefines && refine) HAP_KLAUNCH(kStBcEncode, (bc_encode_kernel<KIND, kRefines>), grid, dim3(kBcThreads), 0, st, rgba, g, blocks);
+    else HAP_KLAUNCH(kStBcEncode, bc_encode_kernel<KIND>, grid, dim3(kBcThreads), 0, st, rgba, g, blocks);
 }
 
 uint32_t launch_block_encode(const uint8_t *rgba, uint32_t frames, uint64_t frame_stride, uint32_t width, uint32_t height,
@@ -331,19 +356,20 @@ uint32_t launch_block_encode(const uint8_t *rgba, uint32_t frames, uint64_t fram
     dim3 grid((g.blocks_x * g.blocks_y + kBcThreads - 1) / kBcThreads, frames);
     const bool refine = g_chroma_refine.load() != 0;
     switch (ci.bc_kind) {
-    case kBcDxt1: HAP_KLAUNCH(kStBcEncode, bc_encode_kernel<kBcDxt1>, grid, dim3(kBcThreads), 0, st, rgba, g, blocks); break;
-    case kBcDxt5: HAP_KLAUNCH(kStBcEncode, bc_encode_kernel<kBcDxt5>, grid, dim3(kBcThreads), 0, st, rgba, g, blocks); break;
-    case kBcYCoCg:
-        if (refine) HAP_KLAUNCH(kStBcEncode, (bc_encode_kernel<kBcYCoCg, true>), grid, dim3(kBcThreads), 0, st, rgba, g, blocks);
-        else HAP_KLAUNCH(kStBcEncode, bc_encode_kernel<kBcYCoCg>, grid, dim3(kBcThreads), 0, st, rgba, g, blocks);
-        break;
-    case kBcRgtc1: HAP_KLAUNCH(kStBcEncode, bc_encode_kernel<kBcRgtc1>, grid, dim3(kBcThreads), 0, st, rgba, g, blocks); break;
-    default:
-        if (refine) HAP_KLAUNCH(kStBcEncode, (bc_encode_kernel<kBcYCoCgPlusAlpha, true>), grid, dim3(kBcThreads), 0, st, rgba, g, blocks);
-        else HAP_KLAUNCH(kStBcEncode, bc_encode_kernel<kBcYCoCgPlusAlpha>, grid, dim3(kBcThreads), 0, st, rgba, g, blocks);
-        break;
+    case kBcDxt1: launch_bc_encode<kBcDxt1>(grid, st, rgba, g, blocks, refine); break;
+    case kBcDxt5: launch_bc_encode<kBcDxt5>(grid, st, rgba, g, blocks, refine); break;
+    case kBcYCoCg: launch_bc_encode<kBcYCoCg>(grid, st, rgba, g, blocks, refine); break;
+    case kBcRgtc1: launch_bc_encode<kBcRgtc1>(grid, st, rgba, g, blocks, refine); break;
+    default: launch_bc_encode<kBcYCoCgPlusAlpha>(grid, st, rgba, g, blocks, refine); break;
     }
     return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
+}
+
+template <int KIND>
+void launch_bc_decode(dim3 grid, cudaStream_t st, const uint8_t *blocks, const uint8_t *alpha, const BcDecodeGeom &g, uint8_t *rgba,
+                      const uint32_t *frame_results)
+{
+    HAP_KLAUNCH(kStBcDecode, bc_decode_kernel<KIND>, grid, dim3(kBcThreads), 0, st, blocks, alpha, g, rgba, frame_results);
 }
 
 uint32_t launch_block_decode(const uint8_t *blocks, const uint8_t *alpha, uint32_t frames, uint64_t blocks_stride,
@@ -360,20 +386,15 @@ uint32_t launch_block_decode(const uint8_t *blocks, const uint8_t *alpha, uint32
     g.frame_bytes = frame_stride;
     dim3 grid((g.blocks_x * g.blocks_y + kBcThreads - 1) / kBcThreads, frames);
     switch (ci.bc_kind) {
-    case kBcDxt1: HAP_KLAUNCH(kStBcDecode, bc_decode_kernel<kBcDxt1>, grid, dim3(kBcThreads), 0, st, blocks, alpha, g, rgba, frame_results); break;
-    case kBcDxt5: HAP_KLAUNCH(kStBcDecode, bc_decode_kernel<kBcDxt5>, grid, dim3(kBcThreads), 0, st, blocks, alpha, g, rgba, frame_results); break;
-    case kBcRgtc1: HAP_KLAUNCH(kStBcDecode, bc_decode_kernel<kBcRgtc1>, grid, dim3(kBcThreads), 0, st, blocks, alpha, g, rgba, frame_results); break;
-    default: HAP_KLAUNCH(kStBcDecode, bc_decode_kernel<kBcYCoCg>, grid, dim3(kBcThreads), 0, st, blocks, alpha, g, rgba, frame_results); break;
+    case kBcDxt1: launch_bc_decode<kBcDxt1>(grid, st, blocks, alpha, g, rgba, frame_results); break;
+    case kBcDxt5: launch_bc_decode<kBcDxt5>(grid, st, blocks, alpha, g, rgba, frame_results); break;
+    case kBcRgtc1: launch_bc_decode<kBcRgtc1>(grid, st, blocks, alpha, g, rgba, frame_results); break;
+    default: launch_bc_decode<kBcYCoCg>(grid, st, blocks, alpha, g, rgba, frame_results); break;   // both scaled-YCoCg kinds
     }
     return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
 }
 
-// Decode-side options (HapB200SetOption): 1 = use a frame's embedded fragment index when it has one (hap_index.h)
-
-// Everything after the jobs exist (device array): windows, on-the-fly index, execute, repair of chunks whose embedded
-// index did not hold up.  in_bound / out_bound: upper bounds of the jobs' total compressed / decoded bytes (they size the
-// window list; a list that turns out too short makes the affected chunks report Internal_Error, never overruns).
-// The decode of a list of chunk jobs: first pass (windows -> on-the-fly index for chunks without one -> execute) and the repair
+// The decode of a list of chunk jobs (a device array): first pass (windows -> on-the-fly index for chunks without one -> execute) and the repair
 // pass for chunks whose embedded index did not describe their stream (decoded again as if they had none).  Batch calls queue
 // both passes (the second finds nothing to do on honest frames); HapDecode, which reads the statuses on the host anyway, only
 // launches the repair pass when a chunk asks for it.
@@ -384,6 +405,8 @@ struct DecodePasses {
     cudaStream_t st;
     explicit DecodePasses(cudaStream_t s) : wins(s), entries(s), done(s), ctl(s), st(s) {}
 
+    // in_bound / out_bound: upper bounds of the jobs' total compressed / decoded bytes (they size the window list; a list
+    // that turns out too short makes the affected chunks report Internal_Error, never overruns)
     uint32_t first(ChunkJob *j, uint32_t n, uint64_t in_bound, uint64_t out_bound)
     {
         jobs = j; njobs = n;
@@ -456,8 +479,9 @@ uint32_t launch_decode_batch(const uint8_t *in, uint32_t frames, uint64_t in_str
 
 // host-side view of a frame whose bytes may live on the device.  Header walks read a few hundred bytes at data-dependent
 // places (section headers, the Decode Instructions tables, five bytes at the head of every chunk, the trailing index header), so
-// a device frame is mirrored LAZILY: `p` points at a zero-page-backed image of the whole frame and need(off, len) fetches the
-// 4 KiB pages under [off, off+len) that are not there yet.  A 4K Hap Q frame costs ~10 small copies instead of 5 MB.
+// a device frame is mirrored LAZILY: `p` points at a zero-page-backed image of the whole frame and need(q, len) fetches the
+// 4 KiB pages under [q, q+len) that are not there yet.  A 4K Hap Q frame costs ~10 small copies instead of 5 MB.  It is the
+// reader the header walks of hap_wire.h take.
 struct HeaderView {
     static constexpr uint64_t kPage = 4096;
     uint8_t *mirror = nullptr;
@@ -468,20 +492,21 @@ struct HeaderView {
     bool ok = true;
     HeaderView(const void *frame, unsigned long n) : bytes(n)
     {
-        if (!is_device_pointer(frame)) { p = (const uint8_t *)frame; return; }
+        if (!is_device(frame)) { p = (const uint8_t *)frame; return; }
         dev = (const uint8_t *)frame;
         mirror = (uint8_t *)calloc(n ? n : 1, 1);     // untouched pages stay uncommitted
         if (!mirror) { ok = false; return; }
         p = mirror;
         have.assign((size_t)((n + kPage - 1) / kPage), false);
-        need(0, kPage);
+        need(p, kPage);
     }
     ~HeaderView() { free(mirror); }
     HeaderView(const HeaderView &) = delete;
     HeaderView &operator=(const HeaderView &) = delete;
-    // make [off, off+len) of the frame readable through p (clamped to the frame); false after a failed copy
-    bool need(uint64_t off, uint64_t len)
+    // make [q, q+len) of the frame readable through p (clamped to the frame); false after a failed copy
+    bool need(const uint8_t *q, uint64_t len)
     {
+        const uint64_t off = (uint64_t)(q - p);
         if (!dev || !ok || off >= bytes || len == 0) return ok;
         if (len > bytes - off) len = bytes - off;
         uint64_t a = off / kPage;
@@ -495,43 +520,6 @@ struct HeaderView {
             a = e;
         }
         return true;
-    }
-    // the texture section `index` (hap.c:932-991), fetching the inner section headers a two-texture frame needs
-    uint32_t locate(uint32_t index, Located &loc)
-    {
-        Section top;
-        if (dev && read_section_header(p, (uint32_t)bytes, top) == HapResult_No_Error && top.type == kSecMultipleImages) {
-            uint64_t off = top.hdr;
-            for (uint32_t i = 0; i < index; i++) {
-                Section s;
-                need(off, 8);
-                if (off >= bytes || read_section_header(p + off, (uint32_t)(bytes - off), s) != HapResult_No_Error) break;
-                off += (uint64_t)s.hdr + s.len;
-            }
-            need(off, 8);
-        }
-        if (!ok) return HapResult_Internal_Error;
-        return locate_texture(p, (uint32_t)bytes, index, loc);
-    }
-    // the Decode Instructions container at the head of texture section `loc` (hap.c:644-730)
-    void need_tables(const Located &loc)
-    {
-        if (!dev) return;
-        need(loc.offset, 8);
-        Section di;
-        if (loc.offset < bytes && read_section_header(p + loc.offset, loc.len, di) == HapResult_No_Error)
-            need(loc.offset, (uint64_t)di.hdr + di.len);
-    }
-    // the trailing fragment index section's header and record-offset table (hap_index.h)
-    void need_index_header()
-    {
-        if (!dev) return;
-        Section top;
-        if (read_section_header(p, (uint32_t)bytes, top) != HapResult_No_Error) return;
-        const uint64_t end = (uint64_t)top.hdr + top.len;
-        need(end, 8 + kIndexHeaderBytes);
-        FragmentIndex ix;
-        if (locate_fragment_index(p, (uint32_t)bytes, ix)) need(ix.body, (uint64_t)kIndexHeaderBytes + 4ull * ((uint64_t)ix.chunks[0] + ix.chunks[1]));
     }
 };
 
@@ -549,23 +537,6 @@ void work_function(void *p, unsigned int)
 
 // ---- delivery rings: helpers ----
 namespace {
-struct OnDevice {      // the calling thread's device for the duration of one ring call
-    int saved = -1;
-    bool ok = false;
-    explicit OnDevice(int device)
-    {
-        if (device < 0 || device >= kMaxDevices || cudaGetDevice(&saved) != cudaSuccess) { cudaGetLastError(); return; }
-        ok = device == saved || cudaSetDevice(device) == cudaSuccess;
-        if (ok) { std::call_once(g_dev[device].once, device_init, device); ok = g_dev[device].ready; }
-        if (!ok) cudaGetLastError();
-    }
-    ~OnDevice()
-    {
-        int cur = -1;
-        if (saved >= 0 && cudaGetDevice(&cur) == cudaSuccess && cur != saved) cudaSetDevice(saved);
-        cudaGetLastError();
-    }
-};
 __global__ void ring_publish_kernel(unsigned int *flag, unsigned int value)
 {
     // the kernels queued before this one have completed, their stores to the peer are performed; the fence orders this
@@ -609,7 +580,7 @@ int HapB200GetDevice(void) { return g_default_device.load(); }
 unsigned int HapB200RingCreate(int device, unsigned long bytes, void **ring, void *handle)
 {
     if (!ring || bytes == 0) return HapResult_Bad_Arguments;
-    OnDevice on(device);
+    DeviceGuard on(device);
     if (!on.ok) return HapResult_Internal_Error;
     void *p = nullptr;
     // plain cudaMalloc: memory of a stream-ordered pool cannot be exported
@@ -631,7 +602,7 @@ unsigned int HapB200RingCreate(int device, unsigned long bytes, void **ring, voi
 unsigned int HapB200RingDestroy(int device, void *ring)
 {
     if (!ring) return HapResult_Bad_Arguments;
-    OnDevice on(device);
+    DeviceGuard on(device);
     if (!on.ok) return HapResult_Internal_Error;
     cudaDeviceSynchronize();
     const bool ok = cudaFree(ring) == cudaSuccess;
@@ -642,7 +613,7 @@ unsigned int HapB200RingDestroy(int device, void *ring)
 unsigned int HapB200RingOpen(int device, const void *handle, void **ring)
 {
     if (!handle || !ring) return HapResult_Bad_Arguments;
-    OnDevice on(device);
+    DeviceGuard on(device);
     if (!on.ok) return HapResult_Internal_Error;
     cudaIpcMemHandle_t h;
     memcpy(&h, handle, sizeof h);
@@ -655,7 +626,7 @@ unsigned int HapB200RingOpen(int device, const void *handle, void **ring)
 unsigned int HapB200RingClose(int device, void *ring)
 {
     if (!ring) return HapResult_Bad_Arguments;
-    OnDevice on(device);
+    DeviceGuard on(device);
     if (!on.ok) return HapResult_Internal_Error;
     cudaDeviceSynchronize();
     const bool ok = cudaIpcCloseMemHandle(ring) == cudaSuccess;
@@ -667,7 +638,7 @@ unsigned int HapB200RingAttach(int device, int ringDevice)
 {
     if (ringDevice < 0 || ringDevice >= kMaxDevices) return HapResult_Bad_Arguments;
     if (device == ringDevice) return HapResult_No_Error;
-    OnDevice on(device);
+    DeviceGuard on(device);
     if (!on.ok) return HapResult_Internal_Error;
     int can = 0;
     if (cudaDeviceCanAccessPeer(&can, device, ringDevice) != cudaSuccess || !can) { cudaGetLastError(); return HapResult_Internal_Error; }
@@ -679,7 +650,7 @@ unsigned int HapB200RingAttach(int device, int ringDevice)
 unsigned int HapB200RingPublish(int device, void *flag, unsigned int value, void *stream)
 {
     if (!flag || ((uintptr_t)flag & 3)) return HapResult_Bad_Arguments;
-    OnDevice on(device);
+    DeviceGuard on(device);
     if (!on.ok) return HapResult_Internal_Error;
     cudaStream_t st = stream ? (cudaStream_t)stream : kLegacyStream;
     ring_publish_kernel<<<1, 1, 0, st>>>((unsigned int *)flag, value);
@@ -690,7 +661,7 @@ unsigned int HapB200RingPublish(int device, void *flag, unsigned int value, void
 unsigned int HapB200RingWait(int device, const void *flag, unsigned int value, unsigned int timeoutMs, void *stream)
 {
     if (!flag || ((uintptr_t)flag & 3)) return HapResult_Bad_Arguments;
-    OnDevice on(device);
+    DeviceGuard on(device);
     if (!on.ok) return HapResult_Internal_Error;
     cudaStream_t st = stream ? (cudaStream_t)stream : kLegacyStream;
     if (timeoutMs == 0) {
@@ -712,15 +683,15 @@ unsigned int HapB200RingWait(int device, const void *flag, unsigned int value, u
     return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
 }
 
-// Options.  HAPB200_OPTION_USE_INDEX (1): decoder uses a frame's embedded fragment index (default 1).
-// HAPB200_OPTION_WRITE_INDEX (2): encoder writes the fragment index section (default: see g_write_index).
 int HapB200SetOption(int option, int value)
 {
-    if (option == 1) { g_use_index.store(value != 0); return 0; }
-    if (option == 2) { g_write_index.store(value != 0); return 0; }
-    if (option == 3) { g_write_offsets.store(value != 0); return 0; }
-    if (option == 4) { g_chroma_refine.store(value != 0); return 0; }
-    return -1;
+    switch (option) {
+    case HAPB200_OPTION_USE_INDEX: g_use_index.store(value != 0); return 0;
+    case HAPB200_OPTION_WRITE_INDEX: g_write_index.store(value != 0); return 0;
+    case HAPB200_OPTION_WRITE_OFFSET_TABLE: g_write_offsets.store(value != 0); return 0;
+    case HAPB200_OPTION_CHROMA_REFINE: g_chroma_refine.store(value != 0); return 0;
+    default: return -1;
+    }
 }
 
 void HapB200SetStageTiming(int enabled)
@@ -731,7 +702,7 @@ void HapB200SetStageTiming(int enabled)
 
 // Synchronises the device, folds the recorded events into per-stage totals and returns them:
 // ms[i], launches[i] for i < n (stage order: bc_encode, snappy_encode, plan, place, parse, snappy_decode,
-// collect, bc_decode).  Totals are reset by the call.
+// collect, bc_decode, snappy_index, windows).  Totals are reset by the call.
 int HapB200StageTimes(double *ms, unsigned long long *launches, int n)
 {
     cudaDeviceSynchronize();
@@ -776,7 +747,7 @@ unsigned int HapGetFrameTextureCount(const void *inputBuffer, unsigned long inpu
     *outputTextureCount = 0;
     while (off < top.len) {  // hap.c:1064 compares against the body length, as here
         Section s;
-        if (!hv.need(off, 8)) return HapResult_Internal_Error;
+        if (!hv.need(in + off, 8)) return HapResult_Internal_Error;
         r = read_section_header(in + off, (uint32_t)(inputBufferBytes - off), s);
         if (r != HapResult_No_Error) return r;
         off += s.hdr + s.len;
@@ -793,7 +764,7 @@ unsigned int HapGetFrameTextureFormat(const void *inputBuffer, unsigned long inp
     HeaderView hv(inputBuffer, inputBufferBytes);
     if (!hv.ok) return HapResult_Internal_Error;
     Located loc;
-    uint32_t r = hv.locate(index, loc);
+    uint32_t r = locate_texture(hv.p, (uint32_t)inputBufferBytes, index, loc, hv);
     if (r != HapResult_No_Error) return r;
     *outputBufferTextureFormat = format_from_nibble(loc.type & 0xF);
     return *outputBufferTextureFormat ? HapResult_No_Error : HapResult_Bad_Frame;
@@ -808,15 +779,13 @@ unsigned int HapGetFrameTextureChunkCount(const void *inputBuffer, unsigned long
     HeaderView hv(inputBuffer, inputBufferBytes);
     if (!hv.ok) return HapResult_Internal_Error;
     Located loc;
-    uint32_t r = hv.locate(index, loc);
+    uint32_t r = locate_texture(hv.p, (uint32_t)inputBufferBytes, index, loc, hv);
     if (r != HapResult_No_Error) return r;
     const uint32_t compressor = (loc.type >> 4) & 0xF;
     if (compressor == kHapComplex) {
         ChunkTables t;
         t.count = 0;
-        hv.need_tables(loc);
-        if (!hv.ok) return HapResult_Internal_Error;
-        r = parse_decode_instructions(hv.p + loc.offset, loc.len, t);
+        r = parse_decode_instructions(hv.p + loc.offset, loc.len, t, hv);
         *chunk_count = t.count;
         return r;
     }
@@ -834,9 +803,7 @@ unsigned int HapEncode(unsigned int count, const void **inputBuffers, unsigned l
         return HapResult_Bad_Arguments;
     for (unsigned i = 0; i < count; i++)
         if (chunkCounts[i] == 0) return HapResult_Bad_Arguments;
-    if (count == 2 && textureFormats[0] != HapFmt_YCoCg_DXT5 && textureFormats[1] != HapFmt_YCoCg_DXT5 &&
-        textureFormats[0] != HapFmt_A_RGTC1 && textureFormats[1] != HapFmt_A_RGTC1)
-        return HapResult_Bad_Arguments;  // hap.c:551-559 (SURVEY.md Q5)
+    if (!texture_formats_ok(count, textureFormats)) return HapResult_Bad_Arguments;
 
     TextureArgs ta[2];
     for (unsigned i = 0; i < count; i++) ta[i] = TextureArgs{inputBuffersBytes[i], textureFormats[i], compressors[i], chunkCounts[i]};
@@ -861,9 +828,9 @@ unsigned int HapEncode(unsigned int count, const void **inputBuffers, unsigned l
         if (gr != HapResult_No_Error) return gr;
     }
 
-    bool all_host_verbatim = !is_device_pointer(outputBuffer);
+    bool all_host_verbatim = !is_device(outputBuffer);
     for (unsigned i = 0; i < count; i++)
-        all_host_verbatim = all_host_verbatim && ta[i].compressor == HapCompressorNone && !is_device_pointer(inputBuffers[i]);
+        all_host_verbatim = all_host_verbatim && ta[i].compressor == HapCompressorNone && !is_device(inputBuffers[i]);
     if (all_host_verbatim) {
         // hap.c:490-501 for every texture: headers plus a copy, nothing to compute and nothing for a GPU to do
         uint8_t *o = (uint8_t *)outputBuffer;
@@ -873,29 +840,18 @@ unsigned int HapEncode(unsigned int count, const void **inputBuffers, unsigned l
             if (i == 1 && (outputBufferBytes < pos ||
                            outputBufferBytes - pos < max_encoded_length_one(ta[1].bytes, ta[1].format, ta[1].compressor, ta[1].chunks)))
                 return HapResult_Buffer_Too_Small;
-            uint8_t h[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-            const uint32_t len = (uint32_t)ta[i].bytes;
-            if (hdr == 4) { h[0] = (uint8_t)len; h[1] = (uint8_t)(len >> 8); h[2] = (uint8_t)(len >> 16); }
-            else { h[4] = (uint8_t)len; h[5] = (uint8_t)(len >> 8); h[6] = (uint8_t)(len >> 16); h[7] = (uint8_t)(len >> 24); }
-            h[3] = (uint8_t)((kHapChunkRaw << 4) | G.s[i].fmt_nibble);
-            memcpy(o + pos, h, hdr);
+            put_section_header(o + pos, hdr, (uint32_t)ta[i].bytes, (kHapChunkRaw << 4) | G.s[i].fmt_nibble);
             memcpy(o + pos + hdr, inputBuffers[i], ta[i].bytes);
             pos += hdr + ta[i].bytes;
         }
-        if (count == 2) {
-            const uint32_t len = (uint32_t)(pos - outer);
-            uint8_t h[8] = {0, 0, 0, (uint8_t)kSecMultipleImages, 0, 0, 0, 0};
-            if (outer == 4) { h[0] = (uint8_t)len; h[1] = (uint8_t)(len >> 8); h[2] = (uint8_t)(len >> 16); }
-            else { h[4] = (uint8_t)len; h[5] = (uint8_t)(len >> 8); h[6] = (uint8_t)(len >> 16); h[7] = (uint8_t)(len >> 24); }
-            memcpy(o, h, outer);
-        }
+        if (count == 2) put_section_header(o, (uint32_t)outer, (uint32_t)(pos - outer), kSecMultipleImages);
         *outputBufferBytesUsed = (unsigned long)pos;
         return HapResult_No_Error;
     }
 
     HAP_ENTER(outputBuffer, inputBuffers[0], count == 2 ? inputBuffers[1] : nullptr);
-    bool enc_all_host = !is_device_pointer(outputBuffer);
-    for (unsigned i = 0; i < count; i++) enc_all_host = enc_all_host && !is_device_pointer(inputBuffers[i]);
+    bool enc_all_host = !is_device(outputBuffer);
+    for (unsigned i = 0; i < count; i++) enc_all_host = enc_all_host && !is_device(inputBuffers[i]);
     CallStream call(enc_all_host);
     cudaStream_t st = call.st;
 
@@ -909,7 +865,7 @@ unsigned int HapEncode(unsigned int count, const void **inputBuffers, unsigned l
     if (!tex.alloc(tex_bytes) || !frame.alloc(cap) || !used.alloc(sizeof(unsigned long long) * 4)) { cudaGetLastError(); return HapResult_Internal_Error; }
     for (unsigned i = 0; i < count; i++) {
         uint8_t *d = tex.as<uint8_t>() + (i ? off1 : 0);
-        cudaMemcpyKind kind = is_device_pointer(inputBuffers[i]) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+        cudaMemcpyKind kind = is_device(inputBuffers[i]) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
         if (cudaMemcpyAsync(d, inputBuffers[i], ta[i].bytes, kind, st) != cudaSuccess) { cudaGetLastError(); return HapResult_Internal_Error; }
         G.s[i].in_offset = i ? off1 : 0;
         G.s[i].in_stride = 0;
@@ -932,7 +888,7 @@ unsigned int HapEncode(unsigned int count, const void **inputBuffers, unsigned l
                 return HapResult_Buffer_Too_Small;
         }
     }
-    cudaMemcpyKind okind = is_device_pointer(outputBuffer) ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+    cudaMemcpyKind okind = is_device(outputBuffer) ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
     if (cudaMemcpyAsync(outputBuffer, frame.p, total, okind, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) {
         cudaGetLastError();
         return HapResult_Internal_Error;
@@ -947,65 +903,19 @@ unsigned int HapDecode(const void *inputBuffer, unsigned long inputBufferBytes, 
                        unsigned long *outputBufferBytesUsed, unsigned int *outputBufferTextureFormat)
 {
     if (!inputBuffer || index > 1 || !callback || !outputBuffer || !outputBufferTextureFormat) return HapResult_Bad_Arguments;
-    const bool in_dev = is_device_pointer(inputBuffer), out_dev = is_device_pointer(outputBuffer);
+    const bool in_dev = is_device(inputBuffer), out_dev = is_device(outputBuffer);
     HeaderView hv(inputBuffer, inputBufferBytes);
     if (!hv.ok) return HapResult_Internal_Error;
-    const uint8_t *frame = hv.p;
-    Located loc;
-    uint32_t r = hv.locate(index, loc);
+    // chunk offsets fit the 32-bit fields of hap.c's HapChunkDecodeInfo
+    TexturePlan plan;
+    std::vector<PlannedJob> planned;
+    uint32_t r = plan_texture(hv.p, (uint32_t)inputBufferBytes, index, outputBufferBytes, ~0u, 0xFFFFFFFFull, hv, plan,
+                              [&](const PlannedJob &j) { planned.push_back(j); });
+    if (plan.located) *outputBufferTextureFormat = plan.format;
     if (r != HapResult_No_Error) return r;
-    const uint8_t *sec = frame + loc.offset;
-    const uint32_t compressor = (loc.type >> 4) & 0xF;
-    *outputBufferTextureFormat = format_from_nibble(loc.type & 0xF);
-    if (*outputBufferTextureFormat == 0) return HapResult_Bad_Frame;
-
-    struct HostJob { uint32_t src_off, src_bytes, dst_off, dst_bytes, compressor, index_off, index_bytes; };
-    std::vector<HostJob> hj;
-    uint32_t hv_index_body = 0, hv_index_len = 0;
-    uint64_t produced = 0;
-    bool whole = false;
-    if (compressor == kHapComplex) {
-        ChunkTables t;
-        t.count = 0;
-        hv.need_tables(loc);
-        if (!hv.ok) return HapResult_Internal_Error;
-        r = parse_decode_instructions(sec, loc.len, t);
-        if (r != HapResult_No_Error) return r;
-        hv.need_index_header();
-        FragmentIndex ix;
-        const bool have_ix = locate_fragment_index(frame, (uint32_t)inputBufferBytes, ix);
-        if (have_ix) { hv_index_body = ix.body; hv_index_len = ix.len; }
-        if (t.count > 0) {
-            uint64_t in_run = 0, out_run = 0;
-            hj.resize((size_t)t.count);
-            for (int i = 0; i < t.count; i++) {
-                const uint32_t cc = sec[t.compressors + i];
-                const uint32_t sz = rd_le32(sec + t.sizes + 4 * i);
-                const uint64_t start = t.data + (t.offsets != 0xFFFFFFFFu ? (uint64_t)rd_le32(sec + t.offsets + 4 * i) : in_run);
-                in_run += sz;
-                if (start + sz > loc.len) return HapResult_Bad_Frame;  // SURVEY.md Q9: the reference reads out of bounds here
-                if (cc == kHapChunkSnappy && !hv.need(loc.offset + start, 5)) return HapResult_Internal_Error;
-                uint32_t usz = sz;
-                if (cc == kHapChunkSnappy && !snappy_preamble(sec + start, sz, usz)) return HapResult_Bad_Frame;  // hap.c:817-829
-                hj[i] = HostJob{(uint32_t)start, sz, 0, usz, (cc == kHapChunkSnappy || cc == kHapChunkRaw) ? cc : 0xFFu, 0, 0};
-                if (cc == kHapChunkSnappy && have_ix) fragment_index_record(frame, ix, index, (uint32_t)t.count, (uint32_t)i, hj[i].index_off, hj[i].index_bytes);
-                if (out_run > 0xFFFFFFFFull) return HapResult_Buffer_Too_Small;
-                hj[i].dst_off = (uint32_t)out_run;
-                out_run += usz;
-            }
-            if (out_run > outputBufferBytes) return HapResult_Buffer_Too_Small;  // hap.c:840-843
-            produced = out_run;
-        }
-    } else if (compressor == kHapChunkSnappy) {
-        uint32_t usz = 0;
-        if (!hv.need(loc.offset, 5)) return HapResult_Internal_Error;
-        if (!snappy_preamble(sec, loc.len, usz)) return HapResult_Internal_Error;  // hap.c:890-894
-        if (usz > outputBufferBytes) return HapResult_Buffer_Too_Small;
-        hj.push_back(HostJob{0, loc.len, 0, usz, kHapChunkSnappy, 0, 0});
-        produced = usz;
-        whole = true;
-    } else if (compressor == kHapChunkRaw) {
-        if (loc.len > outputBufferBytes) return HapResult_Buffer_Too_Small;
+    const Located &loc = plan.loc;
+    const uint8_t *sec = hv.p + loc.offset;
+    if (((loc.type >> 4) & 0xF) == kHapChunkRaw) {
         // hap.c:905-916: a verbatim texture is a copy; nothing to compute
         if (!in_dev && !out_dev) {
             memcpy(outputBuffer, sec, loc.len);
@@ -1016,27 +926,25 @@ unsigned int HapDecode(const void *inputBuffer, unsigned long inputBufferBytes, 
         }
         if (outputBufferBytesUsed) *outputBufferBytesUsed = loc.len;
         return HapResult_No_Error;
-    } else {
-        return HapResult_Bad_Frame;
     }
 
-    if (!hj.empty()) {
+    if (!planned.empty()) {
         HAP_ENTER(inputBuffer, outputBuffer);
         CallStream call(!in_dev && !out_dev);
         cudaStream_t st = call.st;
         DevBuf din(st), dout(st), djobs(st);
         const uint8_t *dsec;
-        const uint8_t *dindex = nullptr;    // device address of byte 0 of the fragment index body (hap_index.h), when the frame has one
+        const uint8_t *dindex = nullptr;    // device address of byte 0 of the fragment index body (hap_index.h), when a chunk has a record
         bool any_index = false;
-        for (auto &h : hj) any_index = any_index || h.index_bytes != 0;
+        for (auto &j : planned) any_index = any_index || j.index_bytes != 0;
         if (in_dev) {
             dsec = (const uint8_t *)inputBuffer + loc.offset;
-            if (any_index) dindex = (const uint8_t *)inputBuffer + hv_index_body;
+            if (any_index) dindex = (const uint8_t *)inputBuffer + plan.ix.body;
         } else {
             // the texture section, and behind it (16-byte aligned) the body of the frame's trailing index section
             const uint64_t ioff = align16(loc.len);
-            if (!din.alloc(ioff + (any_index ? hv_index_len : 0)) || cudaMemcpyAsync(din.p, sec, loc.len, cudaMemcpyHostToDevice, st) != cudaSuccess ||
-                (any_index && cudaMemcpyAsync(din.as<uint8_t>() + ioff, frame + hv_index_body, hv_index_len, cudaMemcpyHostToDevice, st) != cudaSuccess)) {
+            if (!din.alloc(ioff + (any_index ? plan.ix.len : 0)) || cudaMemcpyAsync(din.p, sec, loc.len, cudaMemcpyHostToDevice, st) != cudaSuccess ||
+                (any_index && cudaMemcpyAsync(din.as<uint8_t>() + ioff, hv.p + plan.ix.body, plan.ix.len, cudaMemcpyHostToDevice, st) != cudaSuccess)) {
                 cudaGetLastError();
                 return HapResult_Internal_Error;
             }
@@ -1046,31 +954,28 @@ unsigned int HapDecode(const void *inputBuffer, unsigned long inputBufferBytes, 
         uint8_t *ddst;
         if (out_dev) ddst = (uint8_t *)outputBuffer;
         else {
-            if (!dout.alloc(produced)) { cudaGetLastError(); return HapResult_Internal_Error; }
+            if (!dout.alloc(plan.produced)) { cudaGetLastError(); return HapResult_Internal_Error; }
             ddst = dout.as<uint8_t>();
         }
-        std::vector<ChunkJob> jobs(hj.size());
+        std::vector<ChunkJob> jobs(planned.size());   // (the fields the decode kernels set start zeroed)
         uint64_t in_sum = 0;
-        for (size_t i = 0; i < hj.size(); i++) {
-            jobs[i].src = dsec + hj[i].src_off;
-            jobs[i].dst = ddst + hj[i].dst_off;
-            jobs[i].src_bytes = hj[i].src_bytes;
-            jobs[i].dst_bytes = hj[i].dst_bytes;
-            jobs[i].compressor = hj[i].compressor;
-            jobs[i].status = HapResult_Internal_Error;
-            jobs[i].index = hj[i].index_bytes ? dindex + (hj[i].index_off - hv_index_body) : nullptr;
-            jobs[i].index_bytes = hj[i].index_bytes;
-            jobs[i].mode = kJobUndecided;
-            jobs[i].win_base = 0;
-            jobs[i].win_count = 0;
-            in_sum += hj[i].src_bytes;
+        for (size_t i = 0; i < planned.size(); i++) {
+            const PlannedJob &j = planned[i];
+            jobs[i].src = dsec + (j.src_off - loc.offset);
+            jobs[i].dst = ddst + j.dst_off;
+            jobs[i].src_bytes = j.src_bytes;
+            jobs[i].dst_bytes = j.dst_bytes;
+            jobs[i].compressor = j.compressor;
+            jobs[i].index = j.index_bytes ? dindex + (j.index_off - plan.ix.body) : nullptr;
+            jobs[i].index_bytes = j.index_bytes;
+            in_sum += j.src_bytes;
         }
         if (!djobs.alloc(jobs.size() * sizeof(ChunkJob)) ||
             cudaMemcpyAsync(djobs.p, jobs.data(), jobs.size() * sizeof(ChunkJob), cudaMemcpyHostToDevice, st) != cudaSuccess) { cudaGetLastError(); return HapResult_Internal_Error; }
         DecodePasses passes(st);
-        r = passes.first(djobs.as<ChunkJob>(), (uint32_t)jobs.size(), in_sum, produced);
+        r = passes.first(djobs.as<ChunkJob>(), (uint32_t)jobs.size(), in_sum, plan.produced);
         if (r != HapResult_No_Error) return r;
-        if (compressor == kHapComplex && jobs.size() > 1) {
+        if (!plan.whole && jobs.size() > 1) {
             WorkState ws;
             callback(work_function, &ws, (unsigned)jobs.size(), info);  // hap.c:861
         }
@@ -1085,13 +990,13 @@ unsigned int HapDecode(const void *inputBuffer, unsigned long inputBufferBytes, 
                 cudaStreamSynchronize(st) != cudaSuccess) { cudaGetLastError(); return HapResult_Internal_Error; }
         }
         for (size_t i = 0; i < jobs.size(); i++)
-            if (jobs[i].status != HapResult_No_Error) return whole ? (uint32_t)HapResult_Internal_Error : jobs[i].status;  // hap.c:867-875, :899-903
-        if (!out_dev && produced) {
-            if (cudaMemcpyAsync(outputBuffer, ddst, produced, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+            if (jobs[i].status != HapResult_No_Error) return plan.whole ? (uint32_t)HapResult_Internal_Error : jobs[i].status;  // hap.c:867-875, :899-903
+        if (!out_dev && plan.produced) {
+            if (cudaMemcpyAsync(outputBuffer, ddst, plan.produced, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
                 cudaStreamSynchronize(st) != cudaSuccess) { cudaGetLastError(); return HapResult_Internal_Error; }
         }
     }
-    if (outputBufferBytesUsed) *outputBufferBytesUsed = (unsigned long)produced;
+    if (outputBufferBytesUsed) *outputBufferBytesUsed = (unsigned long)plan.produced;
     return HapResult_No_Error;
 }
 
@@ -1119,15 +1024,14 @@ unsigned int HapB200BlockEncodeBatch(const void *rgba, unsigned int frames, unsi
                                      unsigned long blocksStride, void *stream)
 {
     CodecInfo ci;
-    if (!rgba || !blocks || frames == 0 || !codec_info(codec, ci) || width == 0 || height == 0 || width % 4 || height % 4 ||
-        rowBytes < 4ul * width || rowBytes % 16 || ((uintptr_t)rgba | (uintptr_t)blocks | frameStride | blocksStride) % 16)
+    if (!blocks || frames == 0 || !codec_info(codec, ci) || !rgba_geometry_ok(rgba, width, height, rowBytes, frameStride, true) ||
+        ((uintptr_t)blocks | blocksStride) % 16)
         return HapResult_Bad_Arguments;
     HAP_ENTER(rgba, blocks);
-    cudaStream_t st = stream ? (cudaStream_t)stream : kLegacyStream;
-    uint32_t r = launch_block_encode((const uint8_t *)rgba, frames, frameStride, width, height, rowBytes, ci, (uint8_t *)blocks,
-                                     blocksStride, HapB200TextureBytes(width, height, codec, 0), st);
-    if (r == HapResult_No_Error && !stream && cudaStreamSynchronize(st) != cudaSuccess) { cudaGetLastError(); r = HapResult_Internal_Error; }
-    return r;
+    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
+        return launch_block_encode((const uint8_t *)rgba, frames, frameStride, width, height, rowBytes, ci, (uint8_t *)blocks, blocksStride,
+                                   HapB200TextureBytes(width, height, codec, 0), st);
+    });
 }
 
 unsigned int HapB200BlockDecodeBatch(const void *blocks, unsigned int frames, unsigned long blocksStride, unsigned int width,
@@ -1135,16 +1039,15 @@ unsigned int HapB200BlockDecodeBatch(const void *blocks, unsigned int frames, un
                                      unsigned long rowBytes, void *stream)
 {
     CodecInfo ci;
-    if (!rgba || !blocks || frames == 0 || !codec_info(codec, ci) || width == 0 || height == 0 || width % 4 || height % 4 ||
-        rowBytes < 4ul * width || rowBytes % 16 || ((uintptr_t)rgba | (uintptr_t)blocks | frameStride | blocksStride) % 16)
+    if (!blocks || frames == 0 || !codec_info(codec, ci) || !rgba_geometry_ok(rgba, width, height, rowBytes, frameStride, true) ||
+        ((uintptr_t)blocks | blocksStride) % 16)
         return HapResult_Bad_Arguments;
     HAP_ENTER(blocks, rgba);
-    cudaStream_t st = stream ? (cudaStream_t)stream : kLegacyStream;
     const uint8_t *b = (const uint8_t *)blocks;
-    uint32_t r = launch_block_decode(b, b + HapB200TextureBytes(width, height, codec, 0), frames, blocksStride, blocksStride, width,
-                                     height, ci, (uint8_t *)rgba, frameStride, rowBytes, st);
-    if (r == HapResult_No_Error && !stream && cudaStreamSynchronize(st) != cudaSuccess) { cudaGetLastError(); r = HapResult_Internal_Error; }
-    return r;
+    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
+        return launch_block_decode(b, b + HapB200TextureBytes(width, height, codec, 0), frames, blocksStride, blocksStride, width, height, ci,
+                                   (uint8_t *)rgba, frameStride, rowBytes, st);
+    });
 }
 
 unsigned int HapB200EncodeBatch(unsigned int count, const void **textures, unsigned long *textureStrides,
@@ -1161,23 +1064,18 @@ unsigned int HapB200EncodeBatch(unsigned int count, const void **textures, unsig
         ta[i] = TextureArgs{textureBytes[i], textureFormats[i], compressors[i], chunkCounts[i]};
         if (validate_texture_args(ta[i]) != HapResult_No_Error) return HapResult_Bad_Arguments;
     }
-    if (count == 2 && textureFormats[0] != HapFmt_YCoCg_DXT5 && textureFormats[1] != HapFmt_YCoCg_DXT5 &&
-        textureFormats[0] != HapFmt_A_RGTC1 && textureFormats[1] != HapFmt_A_RGTC1)
-        return HapResult_Bad_Arguments;
+    if (!texture_formats_ok(count, textureFormats)) return HapResult_Bad_Arguments;
     if (outStride < HapMaxEncodedLength(count, textureBytes, textureFormats, chunkCounts)) return HapResult_Buffer_Too_Small;
     FrameGeom G;
     uint32_t r = build_frame_geom(count, ta, G);
     if (r != HapResult_No_Error) return r;
     HAP_ENTER(out, textures[0]);
-    cudaStream_t st = stream ? (cudaStream_t)stream : kLegacyStream;
     const uint8_t *base = (const uint8_t *)textures[0];
     for (unsigned i = 0; i < count; i++) {
         G.s[i].in_offset = (uint64_t)((const uint8_t *)textures[i] - base);  // wraps for i = 1 when below base; 64-bit add undoes it
         G.s[i].in_stride = textureStrides[i];
     }
-    r = launch_encode(base, G, frames, (uint8_t *)out, outStride, used, st);
-    if (r == HapResult_No_Error && !stream && cudaStreamSynchronize(st) != cudaSuccess) { cudaGetLastError(); r = HapResult_Internal_Error; }
-    return r;
+    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t { return launch_encode(base, G, frames, (uint8_t *)out, outStride, used, st); });
 }
 
 unsigned int HapB200EncodeRGBABatch(const void *rgba, unsigned int frames, unsigned long frameStride, unsigned int width,
@@ -1186,31 +1084,29 @@ unsigned int HapB200EncodeRGBABatch(const void *rgba, unsigned int frames, unsig
                                     void *stream)
 {
     CodecInfo ci;
-    if (!rgba || !out || !used || frames == 0 || chunkCount == 0 || !codec_info(codec, ci) || width == 0 || height == 0 ||
-        width % 4 || height % 4 || rowBytes < 4ul * width || rowBytes % 16 || ((uintptr_t)rgba | frameStride) % 16 ||
+    if (!out || !used || frames == 0 || chunkCount == 0 || !codec_info(codec, ci) || !rgba_geometry_ok(rgba, width, height, rowBytes, frameStride, true) ||
         (compressor != HapCompressorNone && compressor != HapCompressorSnappy))
         return HapResult_Bad_Arguments;
     if (outStride < HapB200MaxEncodedLengthRGBA(width, height, codec, chunkCount)) return HapResult_Buffer_Too_Small;
     HAP_ENTER(rgba, out);
-    cudaStream_t st = stream ? (cudaStream_t)stream : kLegacyStream;
-    const uint64_t t0 = HapB200TextureBytes(width, height, codec, 0), t1 = HapB200TextureBytes(width, height, codec, 1);
-    const uint64_t dxt_stride = align16(t0) + align16(t1);
-    DevBuf dxt(st);
-    if (!dxt.alloc(dxt_stride * frames + 16)) { cudaGetLastError(); return HapResult_Internal_Error; }
-    uint32_t r = launch_block_encode((const uint8_t *)rgba, frames, frameStride, width, height, rowBytes, ci, dxt.as<uint8_t>(),
-                                     dxt_stride, align16(t0), st);
-    if (r != HapResult_No_Error) return r;
-    TextureArgs ta[2] = {{t0, ci.fmt[0], compressor, chunkCount}, {t1, ci.fmt[1], compressor, chunkCount}};
-    FrameGeom G;
-    r = build_frame_geom(ci.textures, ta, G);
-    if (r != HapResult_No_Error) return r;
-    for (unsigned i = 0; i < ci.textures; i++) {
-        G.s[i].in_offset = i ? align16(t0) : 0;
-        G.s[i].in_stride = dxt_stride;
-    }
-    r = launch_encode(dxt.as<uint8_t>(), G, frames, (uint8_t *)out, outStride, used, st);
-    if (r == HapResult_No_Error && !stream && cudaStreamSynchronize(st) != cudaSuccess) { cudaGetLastError(); r = HapResult_Internal_Error; }
-    return r;
+    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
+        const uint64_t t0 = HapB200TextureBytes(width, height, codec, 0), t1 = HapB200TextureBytes(width, height, codec, 1);
+        const uint64_t dxt_stride = align16(t0) + align16(t1);
+        DevBuf dxt(st);
+        if (!dxt.alloc(dxt_stride * frames + 16)) { cudaGetLastError(); return (uint32_t)HapResult_Internal_Error; }
+        uint32_t r = launch_block_encode((const uint8_t *)rgba, frames, frameStride, width, height, rowBytes, ci, dxt.as<uint8_t>(),
+                                         dxt_stride, align16(t0), st);
+        if (r != HapResult_No_Error) return r;
+        TextureArgs ta[2] = {{t0, ci.fmt[0], compressor, chunkCount}, {t1, ci.fmt[1], compressor, chunkCount}};
+        FrameGeom G;
+        r = build_frame_geom(ci.textures, ta, G);
+        if (r != HapResult_No_Error) return r;
+        for (unsigned i = 0; i < ci.textures; i++) {
+            G.s[i].in_offset = i ? align16(t0) : 0;
+            G.s[i].in_stride = dxt_stride;
+        }
+        return launch_encode(dxt.as<uint8_t>(), G, frames, (uint8_t *)out, outStride, used, st);
+    });
 }
 
 unsigned int HapB200EncodeRGBA(const void *rgba, unsigned int width, unsigned int height, unsigned long rowBytes,
@@ -1218,14 +1114,13 @@ unsigned int HapB200EncodeRGBA(const void *rgba, unsigned int width, unsigned in
                                unsigned long outputBufferBytes, unsigned long *outputBufferBytesUsed)
 {
     CodecInfo ci;
-    if (!rgba || !outputBuffer || !outputBufferBytesUsed || chunkCount == 0 || !codec_info(codec, ci) || width == 0 ||
-        height == 0 || width % 4 || height % 4 || rowBytes < 4ul * width ||
+    if (!outputBuffer || !outputBufferBytesUsed || chunkCount == 0 || !codec_info(codec, ci) || !rgba_geometry_ok(rgba, width, height, rowBytes, 0, false) ||
         (compressor != HapCompressorNone && compressor != HapCompressorSnappy))
         return HapResult_Bad_Arguments;
     const unsigned long cap = HapB200MaxEncodedLengthRGBA(width, height, codec, chunkCount);
     if (outputBufferBytes < cap) return HapResult_Buffer_Too_Small;
     HAP_ENTER(rgba, outputBuffer);
-    CallStream call(!is_device_pointer(rgba) && !is_device_pointer(outputBuffer));
+    CallStream call(!is_device(rgba) && !is_device(outputBuffer));
     cudaStream_t st = call.st;
     DevBuf img(st), frame(st), used(st);
     const uint64_t tight = 4ull * width;
@@ -1249,11 +1144,10 @@ unsigned int HapB200DecodeBatch(const void *in, unsigned int frames, unsigned lo
     if (!in || !inBytes || !out || !used || !formats || !results || frames == 0 || maxChunks == 0 || index > 1)
         return HapResult_Bad_Arguments;
     HAP_ENTER(in, out);
-    cudaStream_t st = stream ? (cudaStream_t)stream : kLegacyStream;
-    uint32_t r = launch_decode_batch((const uint8_t *)in, frames, inStride, inBytes, index, maxChunks, (uint8_t *)out, outStride, outStride,
-                                     used, formats, results, st);
-    if (r == HapResult_No_Error && !stream && cudaStreamSynchronize(st) != cudaSuccess) { cudaGetLastError(); r = HapResult_Internal_Error; }
-    return r;
+    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
+        return launch_decode_batch((const uint8_t *)in, frames, inStride, inBytes, index, maxChunks, (uint8_t *)out, outStride, outStride,
+                                   used, formats, results, st);
+    });
 }
 
 unsigned int HapB200DecodeRGBABatch(const void *in, unsigned int frames, unsigned long inStride, const unsigned long long *inBytes,
@@ -1261,61 +1155,52 @@ unsigned int HapB200DecodeRGBABatch(const void *in, unsigned int frames, unsigne
                                     unsigned long frameStride, unsigned long rowBytes, unsigned int *results, void *stream)
 {
     CodecInfo ci;
-    if (!in || !inBytes || !rgba || !results || frames == 0 || maxChunks == 0 || !codec_info(codec, ci) || width == 0 ||
-        height == 0 || width % 4 || height % 4 || rowBytes < 4ul * width || rowBytes % 16 || ((uintptr_t)rgba | frameStride) % 16)
+    if (!in || !inBytes || !results || frames == 0 || maxChunks == 0 || !codec_info(codec, ci) ||
+        !rgba_geometry_ok(rgba, width, height, rowBytes, frameStride, true))
         return HapResult_Bad_Arguments;
     HAP_ENTER(in, rgba);
-    cudaStream_t st = stream ? (cudaStream_t)stream : kLegacyStream;
-    const uint64_t t0 = HapB200TextureBytes(width, height, codec, 0), t1 = HapB200TextureBytes(width, height, codec, 1);
-    const uint64_t dxt_stride = align16(t0) + align16(t1);
-    DevBuf dxt(st), used(st), formats(st), res1(st);
-    if (!dxt.alloc(dxt_stride * frames + 16) || !used.alloc(8ull * frames) || !formats.alloc(4ull * frames) || !res1.alloc(4ull * frames)) {
-        cudaGetLastError();
-        return HapResult_Internal_Error;
-    }
-    uint32_t r = HapResult_No_Error;
-    for (uint32_t ti = 0; ti < ci.textures && r == HapResult_No_Error; ti++) {
-        uint32_t *res = ti == 0 ? results : res1.as<uint32_t>();
-        // the decoded size must equal the texture size: offer exactly that much room per frame (the slot stride is
-        // wider: both textures of a frame share a slot, so a texture that over-declares its size must not reach its
-        // neighbour or the next frame's slot)
-        r = launch_decode_batch((const uint8_t *)in, frames, inStride, inBytes, ti, maxChunks, dxt.as<uint8_t>() + (ti ? align16(t0) : 0),
-                                dxt_stride, ti ? t1 : t0, used.as<unsigned long long>(), formats.as<uint32_t>(), res, st);
-        if (r != HapResult_No_Error) break;
-        HAP_KLAUNCH(kStCollect, hap_check_texture_kernel, dim3((frames + 127) / 128), dim3(128), 0, st, frames, used.as<unsigned long long>(),
-                    formats.as<uint32_t>(), res, (unsigned long long)(ti ? t1 : t0), ci.fmt[ti], results);
-    }
-    if (r == HapResult_No_Error)
-        r = launch_block_decode(dxt.as<uint8_t>(), dxt.as<uint8_t>() + align16(t0), frames, dxt_stride, dxt_stride, width, height, ci,
-                                (uint8_t *)rgba, frameStride, rowBytes, st, results);
-    if (r == HapResult_No_Error && !stream && cudaStreamSynchronize(st) != cudaSuccess) { cudaGetLastError(); r = HapResult_Internal_Error; }
-    return r;
+    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
+        const uint64_t t0 = HapB200TextureBytes(width, height, codec, 0), t1 = HapB200TextureBytes(width, height, codec, 1);
+        const uint64_t dxt_stride = align16(t0) + align16(t1);
+        DevBuf dxt(st), used(st), formats(st), res1(st);
+        if (!dxt.alloc(dxt_stride * frames + 16) || !used.alloc(8ull * frames) || !formats.alloc(4ull * frames) || !res1.alloc(4ull * frames)) {
+            cudaGetLastError();
+            return HapResult_Internal_Error;
+        }
+        for (uint32_t ti = 0; ti < ci.textures; ti++) {
+            uint32_t *res = ti == 0 ? results : res1.as<uint32_t>();
+            // the decoded size must equal the texture size: offer exactly that much room per frame (the slot stride is
+            // wider: both textures of a frame share a slot, so a texture that over-declares its size must not reach its
+            // neighbour or the next frame's slot)
+            const uint32_t r = launch_decode_batch((const uint8_t *)in, frames, inStride, inBytes, ti, maxChunks, dxt.as<uint8_t>() + (ti ? align16(t0) : 0),
+                                                   dxt_stride, ti ? t1 : t0, used.as<unsigned long long>(), formats.as<uint32_t>(), res, st);
+            if (r != HapResult_No_Error) return r;
+            HAP_KLAUNCH(kStCollect, hap_check_texture_kernel, dim3((frames + 127) / 128), dim3(128), 0, st, frames, used.as<unsigned long long>(),
+                        formats.as<uint32_t>(), res, (unsigned long long)(ti ? t1 : t0), ci.fmt[ti], results);
+        }
+        return launch_block_decode(dxt.as<uint8_t>(), dxt.as<uint8_t>() + align16(t0), frames, dxt_stride, dxt_stride, width, height, ci,
+                                   (uint8_t *)rgba, frameStride, rowBytes, st, results);
+    });
 }
 
 unsigned int HapB200DecodeRGBA(const void *inputBuffer, unsigned long inputBufferBytes, unsigned int width, unsigned int height,
                                void *rgba, unsigned long rowBytes)
 {
-    if (!inputBuffer || !rgba || width == 0 || height == 0 || width % 4 || height % 4 || rowBytes < 4ul * width)
-        return HapResult_Bad_Arguments;
+    if (!inputBuffer || !rgba_geometry_ok(rgba, width, height, rowBytes, 0, false)) return HapResult_Bad_Arguments;
     unsigned count = 0, f0 = 0, f1 = 0;
     uint32_t r = HapGetFrameTextureCount(inputBuffer, inputBufferBytes, &count);
     if (r != HapResult_No_Error) return r;
     r = HapGetFrameTextureFormat(inputBuffer, inputBufferBytes, 0, &f0);
     if (r != HapResult_No_Error) return r;
-    unsigned codec;
     if (count == 2) {
         r = HapGetFrameTextureFormat(inputBuffer, inputBufferBytes, 1, &f1);
         if (r != HapResult_No_Error) return r;
-        if (f0 != HapFmt_YCoCg_DXT5 || f1 != HapFmt_A_RGTC1) return HapResult_Bad_Frame;
-        codec = HapB200Codec_HapM;
-    } else if (count == 1) {
-        codec = f0 == HapFmt_RGB_DXT1 ? HapB200Codec_Hap1 : f0 == HapFmt_RGBA_DXT5 ? HapB200Codec_Hap5 :
-                f0 == HapFmt_YCoCg_DXT5 ? HapB200Codec_HapY : f0 == HapFmt_A_RGTC1 ? HapB200Codec_HapA : 99u;
-    } else {
-        return HapResult_Bad_Frame;
     }
+    // the codec whose textures the frame has (BPTC frames carry no RGBA decoder here)
+    unsigned codec = 0;
     CodecInfo ci;
-    if (!codec_info(codec, ci)) return HapResult_Bad_Frame;  // BPTC frames carry no RGBA decoder here
+    while (codec_info(codec, ci) && (ci.textures != count || ci.fmt[0] != f0 || (count == 2 && ci.fmt[1] != f1))) codec++;
+    if (!codec_info(codec, ci)) return HapResult_Bad_Frame;
     HAP_ENTER(inputBuffer, rgba);
     const uint64_t t0 = HapB200TextureBytes(width, height, codec, 0), t1 = HapB200TextureBytes(width, height, codec, 1);
     const uint64_t tight = 4ull * width;

@@ -12,6 +12,7 @@
 //                            padding, exactly as hap.c:473 lays them out.
 #pragma once
 #include "block_primitives.cuh"
+#include "hap_wire.h"
 #include "snappy_encode.cuh"
 
 namespace hapb200 {
@@ -19,18 +20,6 @@ namespace hapb200 {
 constexpr int kPlanThreads = 256;
 constexpr uint32_t kPlanWriteIndex = 1, kPlanWriteOffsets = 2;
 constexpr uint32_t kPlaceRawFlag = 0x80000000u;
-
-__device__ __forceinline__ void put_section_header(uint8_t *p, uint32_t hdr, uint32_t len, uint32_t type)
-{
-    // hap.c:189-212
-    if (hdr == 4) {
-        p[0] = (uint8_t)len; p[1] = (uint8_t)(len >> 8); p[2] = (uint8_t)(len >> 16);
-    } else {
-        p[0] = p[1] = p[2] = 0;
-        p[4] = (uint8_t)len; p[5] = (uint8_t)(len >> 8); p[6] = (uint8_t)(len >> 16); p[7] = (uint8_t)(len >> 24);
-    }
-    p[3] = (uint8_t)type;
-}
 
 __device__ __forceinline__ uint32_t varint_bytes(uint32_t v) { return v < (1u << 7) ? 1 : v < (1u << 14) ? 2 : v < (1u << 21) ? 3 : v < (1u << 28) ? 4 : 5; }
 

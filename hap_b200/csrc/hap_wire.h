@@ -18,6 +18,32 @@ struct Section {
     uint32_t hdr, len, type;
 };
 
+// The header walks below call need(p, len) before they read [p, p+len) of a frame; false means the bytes could not be
+// fetched (the walk then fails with Internal_Error).  Frames the caller can read directly use NoFetch; the host entry
+// points reading a device frame pass a reader that copies the bytes over on demand (hap_api.cu HeaderView).
+struct NoFetch {
+    HAP_HD bool need(const uint8_t *, uint64_t) const { return true; }
+};
+// Precedes the templates that call their reader (or a sink, hap_parse.cuh): instantiated for the host, they may call
+// host-only code.
+#if defined(__CUDACC__) && !defined(HAPB200_EMU)
+#define HAP_HD_TEMPLATE _Pragma("nv_exec_check_disable")
+#else
+#define HAP_HD_TEMPLATE
+#endif
+
+// hap.c:189-212: a 4- or 8-byte section header at p
+HAP_HD void put_section_header(uint8_t *p, uint32_t hdr, uint32_t len, uint32_t type)
+{
+    if (hdr == 4) {
+        p[0] = (uint8_t)len; p[1] = (uint8_t)(len >> 8); p[2] = (uint8_t)(len >> 16);
+    } else {
+        p[0] = p[1] = p[2] = 0;
+        p[4] = (uint8_t)len; p[5] = (uint8_t)(len >> 8); p[6] = (uint8_t)(len >> 16); p[7] = (uint8_t)(len >> 24);
+    }
+    p[3] = (uint8_t)type;
+}
+
 // hap.c:137-187.  The reference does this arithmetic in 32 bits (hap.c:181); `avail` is truncated
 // the same way by the callers (hap.c:1022 -> :932).
 HAP_HD uint32_t read_section_header(const uint8_t *p, uint32_t avail, Section &s)
@@ -69,9 +95,12 @@ HAP_HD uint32_t nibble_from_format(uint32_t fmt)
 struct Located {
     uint32_t offset, len, type;
 };
-HAP_HD uint32_t locate_texture(const uint8_t *in, uint32_t n, uint32_t index, Located &out)
+HAP_HD_TEMPLATE
+template <class Reader = NoFetch>
+HAP_HD uint32_t locate_texture(const uint8_t *in, uint32_t n, uint32_t index, Located &out, Reader &&rd = Reader())
 {
     Section top;
+    if (!rd.need(in, 8)) return HapResult_Internal_Error;
     uint32_t r = read_section_header(in, n, top);
     if (r != HapResult_No_Error) return r;
     if (top.type == kSecMultipleImages) {
@@ -81,6 +110,7 @@ HAP_HD uint32_t locate_texture(const uint8_t *in, uint32_t n, uint32_t index, Lo
         for (uint32_t i = 0; i <= index; i++) {
             off += (uint64_t)cur.hdr + cur.len;
             if (off >= top.len) return HapResult_Bad_Arguments;
+            if (!rd.need(in + top.hdr + off, 8)) return HapResult_Internal_Error;
             r = read_section_header(in + top.hdr + off, (uint32_t)(top.len - off), cur);
             if (r != HapResult_No_Error) return r;
         }
@@ -105,15 +135,19 @@ struct ChunkTables {
     int count;
     bool has_compressors, has_sizes;
 };
-HAP_HD uint32_t parse_decode_instructions(const uint8_t *sec, uint32_t sec_len, ChunkTables &t)
+HAP_HD_TEMPLATE
+template <class Reader = NoFetch>
+HAP_HD uint32_t parse_decode_instructions(const uint8_t *sec, uint32_t sec_len, ChunkTables &t, Reader &&rd = Reader())
 {
     // t.count is an in/out accumulator exactly like the reference's int *chunk_count
     t.has_compressors = t.has_sizes = false;
     t.offsets = 0xFFFFFFFFu;
     Section s;
+    if (!rd.need(sec, 8)) return HapResult_Internal_Error;
     uint32_t r = read_section_header(sec, sec_len, s);
     if (r == HapResult_No_Error && s.type != kSecDecodeInstructions) r = HapResult_Bad_Frame;
     if (r != HapResult_No_Error) return r;
+    if (!rd.need(sec, (uint64_t)s.hdr + s.len)) return HapResult_Internal_Error;   // the whole container: tables included
     t.data = s.hdr + s.len;
     uint32_t pos = s.hdr, left = s.len;
     // byte lengths of the tables as found (0xFFFFFFFF = table absent): the entry counts derived from them must all
@@ -152,12 +186,14 @@ struct FragmentIndex {
     uint32_t body, len;
     uint32_t chunks[2];
 };
-HAP_HD bool locate_fragment_index(const uint8_t *frame, uint32_t n, FragmentIndex &ix)
+HAP_HD_TEMPLATE
+template <class Reader = NoFetch>
+HAP_HD bool locate_fragment_index(const uint8_t *frame, uint32_t n, FragmentIndex &ix, Reader &&rd = Reader())
 {
     Section top;
-    if (read_section_header(frame, n, top) != HapResult_No_Error) return false;
+    if (!rd.need(frame, 8) || read_section_header(frame, n, top) != HapResult_No_Error) return false;
     const uint64_t end = (uint64_t)top.hdr + top.len;
-    if (end + 4 > n) return false;
+    if (end + 4 > n || !rd.need(frame + end, 8 + kIndexHeaderBytes)) return false;
     Section s;
     if (read_section_header(frame + end, (uint32_t)(n - end), s) != HapResult_No_Error || s.type != kSecFragmentIndex) return false;
     if (s.len < kIndexHeaderBytes) return false;
@@ -167,8 +203,8 @@ HAP_HD bool locate_fragment_index(const uint8_t *frame, uint32_t n, FragmentInde
     ix.len = s.len;
     ix.chunks[0] = rd_le32(b + 12);
     ix.chunks[1] = rd_le32(b + 16);
-    if ((uint64_t)kIndexHeaderBytes + 4ull * ((uint64_t)ix.chunks[0] + ix.chunks[1]) > s.len) return false;
-    return true;
+    const uint64_t table = (uint64_t)kIndexHeaderBytes + 4ull * ((uint64_t)ix.chunks[0] + ix.chunks[1]);
+    return table <= s.len && rd.need(b, table);     // fragment_index_record reads the record-offset table
 }
 // The record of chunk `i` of texture `texture` (which has `count` chunks by its own tables): offset from the frame start
 // and the bytes readable from there; false when there is no record for it.

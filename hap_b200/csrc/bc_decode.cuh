@@ -158,7 +158,21 @@ struct BcDecodeGeom {
     uint64_t frame_bytes;    // RGBA frame stride
 };
 
-// grid = (ceil(blocks/kBcThreads), frames).  kBcRgtc1 alone writes the value to all of R,G,B with A=255.
+HAP_HD BcDecodeGeom bc_decode_geom(uint32_t width, uint32_t height, uint32_t row_bytes, bool merge_alpha, uint64_t in_stride,
+                                   uint64_t alpha_stride, uint64_t frame_bytes)
+{
+    BcDecodeGeom g;
+    g.blocks_x = width / 4;
+    g.blocks_y = height / 4;
+    g.row_bytes = row_bytes;
+    g.merge_alpha = merge_alpha ? 1u : 0u;
+    g.in_stride = in_stride;
+    g.alpha_stride = alpha_stride;
+    g.frame_bytes = frame_bytes;
+    return g;
+}
+
+// grid = (bc_ctas, frames).  kBcRgtc1 alone writes the value to all of R,G,B with A=255.
 template <int KIND>
 __global__ void __launch_bounds__(kBcThreads) bc_decode_kernel(const uint8_t *__restrict__ blocks,
                                                                 const uint8_t *__restrict__ alpha_blocks,

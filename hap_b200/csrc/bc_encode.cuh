@@ -28,7 +28,29 @@ struct BcGeom {
     uint64_t second_offset;        // kBcYCoCgPlusAlpha: offset of the RGTC1 plane inside a frame's output
 };
 
-// grid = (ceil(blocks/kBcThreads), frames).  REFINE: the chroma endpoint refinement of the YCoCg kinds (bc_block.cuh).
+// The geometry of width x height pictures (multiples of 4, at most 2^32 - 1 blocks), rows row_bytes apart.
+HAP_HD BcGeom bc_encode_geom(uint32_t width, uint32_t height, uint32_t row_bytes, uint64_t frame_bytes, uint64_t out_stride,
+                             uint64_t second_offset)
+{
+    BcGeom g;
+    g.blocks_x = width / 4;
+    g.blocks_y = height / 4;
+    g.row_bytes = row_bytes;
+    const uint64_t inv = 0x100000000ull / g.blocks_x;          // 2^32 when the image is one block wide
+    g.inv_blocks_x = inv > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)inv;
+    g.frame_bytes = frame_bytes;
+    g.out_stride = out_stride;
+    g.second_offset = second_offset;
+    return g;
+}
+
+// CTAs per frame of the block kernels (encode and decode): one thread per block
+HAP_HD uint32_t bc_ctas(uint32_t blocks_x, uint32_t blocks_y) { return (uint32_t)(((uint64_t)blocks_x * blocks_y + kBcThreads - 1) / kBcThreads); }
+
+// The frame is blockIdx.y, and gridDim.y is at most 65535: batches of more frames are launched in slices of this many.
+constexpr uint32_t kBcFramesPerLaunch = 65535;
+
+// grid = (bc_ctas, frames).  REFINE: the chroma endpoint refinement of the YCoCg kinds (bc_block.cuh).
 template <int KIND, bool REFINE = false>
 __global__ void __launch_bounds__(kBcThreads, (KIND == kBcYCoCg && !REFINE) ? 7 : (KIND == kBcDxt1 || KIND == kBcDxt5) ? 5 : HAPB200_BC_MIN_BLOCKS) bc_encode_kernel(const uint8_t *__restrict__ rgba, BcGeom G,
                                                                 uint8_t *__restrict__ out)

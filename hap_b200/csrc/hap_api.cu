@@ -281,10 +281,11 @@ bool texture_formats_ok(unsigned count, const unsigned *f)
 }
 
 // width x height RGBA pictures, rows rowBytes apart.  aligned: the batch entry points' rules besides (16-byte aligned rows,
-// picture address and picture stride).
+// picture address and picture stride).  The block kernels hold the row pitch and the block index in 32 bits.
 bool rgba_geometry_ok(const void *rgba, unsigned width, unsigned height, unsigned long rowBytes, unsigned long frameStride, bool aligned)
 {
     if (!rgba || width == 0 || height == 0 || width % 4 || height % 4 || rowBytes < 4ul * width) return false;
+    if (rowBytes > HAPB200_MAX_ROW_BYTES || (unsigned long)(width / 4) * (height / 4) > HAPB200_MAX_BLOCKS) return false;
     return !aligned || (rowBytes % 16 == 0 && ((uintptr_t)rgba | frameStride) % 16 == 0);
 }
 
@@ -331,65 +332,57 @@ uint32_t launch_encode(const uint8_t *base, const FrameGeom &G, uint32_t frames,
     return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
 }
 
-// the scaled-YCoCg kinds have a chroma-refining variant (HAPB200_OPTION_CHROMA_REFINE)
+// the scaled-YCoCg kinds have a chroma-refining variant (HAPB200_OPTION_CHROMA_REFINE).  One launch per kBcFramesPerLaunch frames.
 template <int KIND>
-void launch_bc_encode(dim3 grid, cudaStream_t st, const uint8_t *rgba, const BcGeom &g, uint8_t *blocks, bool refine)
+void launch_bc_encode(uint32_t frames, cudaStream_t st, const uint8_t *rgba, const BcGeom &g, uint8_t *blocks, bool refine)
 {
     constexpr bool kRefines = KIND == kBcYCoCg || KIND == kBcYCoCgPlusAlpha;
-    if (kRefines && refine) HAP_KLAUNCH(kStBcEncode, (bc_encode_kernel<KIND, kRefines>), grid, dim3(kBcThreads), 0, st, rgba, g, blocks);
-    else HAP_KLAUNCH(kStBcEncode, bc_encode_kernel<KIND>, grid, dim3(kBcThreads), 0, st, rgba, g, blocks);
+    for (uint32_t f0 = 0; f0 < frames; f0 += kBcFramesPerLaunch) {
+        const dim3 grid(bc_ctas(g.blocks_x, g.blocks_y), frames - f0 < kBcFramesPerLaunch ? frames - f0 : kBcFramesPerLaunch);
+        const uint8_t *src = rgba + f0 * g.frame_bytes;
+        uint8_t *dst = blocks + f0 * g.out_stride;
+        if (kRefines && refine) HAP_KLAUNCH(kStBcEncode, (bc_encode_kernel<KIND, kRefines>), grid, dim3(kBcThreads), 0, st, src, g, dst);
+        else HAP_KLAUNCH(kStBcEncode, bc_encode_kernel<KIND>, grid, dim3(kBcThreads), 0, st, src, g, dst);
+    }
 }
 
 uint32_t launch_block_encode(const uint8_t *rgba, uint32_t frames, uint64_t frame_stride, uint32_t width, uint32_t height,
                              uint64_t row_bytes, const CodecInfo &ci, uint8_t *blocks, uint64_t blocks_stride,
                              uint64_t second_offset, cudaStream_t st)
 {
-    BcGeom g;
-    g.blocks_x = width / 4;
-    g.blocks_y = height / 4;
-    g.row_bytes = (uint32_t)row_bytes;
-    const uint64_t inv = 0x100000000ull / g.blocks_x;          // 2^32 when the image is one block wide
-    g.inv_blocks_x = inv > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)inv;
-    g.frame_bytes = frame_stride;
-    g.out_stride = blocks_stride;
-    g.second_offset = second_offset;
-    dim3 grid((g.blocks_x * g.blocks_y + kBcThreads - 1) / kBcThreads, frames);
+    const BcGeom g = bc_encode_geom(width, height, (uint32_t)row_bytes, frame_stride, blocks_stride, second_offset);   // (rgba_geometry_ok: row_bytes < 2^32)
     const bool refine = g_chroma_refine.load() != 0;
     switch (ci.bc_kind) {
-    case kBcDxt1: launch_bc_encode<kBcDxt1>(grid, st, rgba, g, blocks, refine); break;
-    case kBcDxt5: launch_bc_encode<kBcDxt5>(grid, st, rgba, g, blocks, refine); break;
-    case kBcYCoCg: launch_bc_encode<kBcYCoCg>(grid, st, rgba, g, blocks, refine); break;
-    case kBcRgtc1: launch_bc_encode<kBcRgtc1>(grid, st, rgba, g, blocks, refine); break;
-    default: launch_bc_encode<kBcYCoCgPlusAlpha>(grid, st, rgba, g, blocks, refine); break;
+    case kBcDxt1: launch_bc_encode<kBcDxt1>(frames, st, rgba, g, blocks, refine); break;
+    case kBcDxt5: launch_bc_encode<kBcDxt5>(frames, st, rgba, g, blocks, refine); break;
+    case kBcYCoCg: launch_bc_encode<kBcYCoCg>(frames, st, rgba, g, blocks, refine); break;
+    case kBcRgtc1: launch_bc_encode<kBcRgtc1>(frames, st, rgba, g, blocks, refine); break;
+    default: launch_bc_encode<kBcYCoCgPlusAlpha>(frames, st, rgba, g, blocks, refine); break;
     }
     return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
 }
 
 template <int KIND>
-void launch_bc_decode(dim3 grid, cudaStream_t st, const uint8_t *blocks, const uint8_t *alpha, const BcDecodeGeom &g, uint8_t *rgba,
+void launch_bc_decode(uint32_t frames, cudaStream_t st, const uint8_t *blocks, const uint8_t *alpha, const BcDecodeGeom &g, uint8_t *rgba,
                       const uint32_t *frame_results)
 {
-    HAP_KLAUNCH(kStBcDecode, bc_decode_kernel<KIND>, grid, dim3(kBcThreads), 0, st, blocks, alpha, g, rgba, frame_results);
+    for (uint32_t f0 = 0; f0 < frames; f0 += kBcFramesPerLaunch) {
+        const dim3 grid(bc_ctas(g.blocks_x, g.blocks_y), frames - f0 < kBcFramesPerLaunch ? frames - f0 : kBcFramesPerLaunch);
+        HAP_KLAUNCH(kStBcDecode, bc_decode_kernel<KIND>, grid, dim3(kBcThreads), 0, st, blocks + f0 * g.in_stride, alpha + f0 * g.alpha_stride, g,
+                    rgba + f0 * g.frame_bytes, frame_results ? frame_results + f0 : nullptr);
+    }
 }
 
 uint32_t launch_block_decode(const uint8_t *blocks, const uint8_t *alpha, uint32_t frames, uint64_t blocks_stride,
                              uint64_t alpha_stride, uint32_t width, uint32_t height, const CodecInfo &ci, uint8_t *rgba,
                              uint64_t frame_stride, uint64_t row_bytes, cudaStream_t st, const uint32_t *frame_results = nullptr)
 {
-    BcDecodeGeom g;
-    g.blocks_x = width / 4;
-    g.blocks_y = height / 4;
-    g.row_bytes = (uint32_t)row_bytes;
-    g.merge_alpha = ci.textures == 2;
-    g.in_stride = blocks_stride;
-    g.alpha_stride = alpha_stride;
-    g.frame_bytes = frame_stride;
-    dim3 grid((g.blocks_x * g.blocks_y + kBcThreads - 1) / kBcThreads, frames);
+    const BcDecodeGeom g = bc_decode_geom(width, height, (uint32_t)row_bytes, ci.textures == 2, blocks_stride, alpha_stride, frame_stride);
     switch (ci.bc_kind) {
-    case kBcDxt1: launch_bc_decode<kBcDxt1>(grid, st, blocks, alpha, g, rgba, frame_results); break;
-    case kBcDxt5: launch_bc_decode<kBcDxt5>(grid, st, blocks, alpha, g, rgba, frame_results); break;
-    case kBcRgtc1: launch_bc_decode<kBcRgtc1>(grid, st, blocks, alpha, g, rgba, frame_results); break;
-    default: launch_bc_decode<kBcYCoCg>(grid, st, blocks, alpha, g, rgba, frame_results); break;   // both scaled-YCoCg kinds
+    case kBcDxt1: launch_bc_decode<kBcDxt1>(frames, st, blocks, alpha, g, rgba, frame_results); break;
+    case kBcDxt5: launch_bc_decode<kBcDxt5>(frames, st, blocks, alpha, g, rgba, frame_results); break;
+    case kBcRgtc1: launch_bc_decode<kBcRgtc1>(frames, st, blocks, alpha, g, rgba, frame_results); break;
+    default: launch_bc_decode<kBcYCoCg>(frames, st, blocks, alpha, g, rgba, frame_results); break;   // both scaled-YCoCg kinds
     }
     return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
 }

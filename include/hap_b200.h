@@ -99,6 +99,12 @@ unsigned long HapB200MaxEncodedLengthRGBA(unsigned int width, unsigned int heigh
 /* bytes of texture `index` (0 or 1) of a width x height frame of `codec`; 0 when absent */
 unsigned long HapB200TextureBytes(unsigned int width, unsigned int height, unsigned int codec, unsigned int index);
 
+/* Limits of every RGBA picture below (HapB200EncodeRGBA .. HapB200BlockDecodeBatch): rowBytes is at most
+ * HAPB200_MAX_ROW_BYTES and (width/4)*(height/4) at most HAPB200_MAX_BLOCKS; larger values are refused with
+ * HapResult_Bad_Arguments.  A batch may hold any number of frames. */
+#define HAPB200_MAX_ROW_BYTES 0xFFFFFFFFul
+#define HAPB200_MAX_BLOCKS 0xFFFFFFFFul
+
 /* One RGBA8 frame (row-major, rowBytes stride, width/height multiples of 4) -> one Hap frame.
  * Host or device pointers.  Fuses block compression, Snappy and frame assembly on the GPU. */
 unsigned int HapB200EncodeRGBA(const void *rgba, unsigned int width, unsigned int height, unsigned long rowBytes,

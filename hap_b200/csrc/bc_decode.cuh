@@ -1,4 +1,4 @@
-// hap_b200/csrc/bc_decode.cuh -- K8: DXT1 / DXT5 / scaled-YCoCg-DXT5 / RGTC1 blocks -> RGBA8.
+// hap_b200/csrc/bc_decode.cuh -- K8: DXT1 / DXT5 / scaled-YCoCg-DXT5 / RGTC1 / BC7 blocks -> RGBA8.
 //
 // The step AFTER HapDecode in every player: in the reference's world it is the GPU texture unit plus
 // a YCoCg fragment shader (/root/reference/README.md:4, documentation/HapVideoDRAFT.md:8,81).  Here it
@@ -8,6 +8,7 @@
 // One thread per block: reads 8/16 contiguous bytes, writes four 16-byte row pieces; a warp therefore
 // writes 512 contiguous bytes per pixel row.
 #pragma once
+#include "bc7_decode.cuh"
 #include "bc_encode.cuh"
 
 namespace hapb200 {
@@ -102,6 +103,10 @@ HAP_HD void interleave_rows(const uint32_t R[4], const uint32_t G[4], const uint
 // texel t of a decoded block; out[16] packed RGBA (kBcRgtc1: the value in every colour channel, A = 255)
 HAP_HD void decode_block(int kind, uint32_t w0, uint32_t w1, uint32_t w2, uint32_t w3, uint32_t out[16])
 {
+    if (kind == kBcBc7) {
+        bc7_decode_block(w0, w1, w2, w3, out);
+        return;
+    }
     const uint32_t ones[4] = {0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu};
     if (kind == kBcDxt1) {
         uint32_t ch[4][4];
@@ -172,7 +177,7 @@ HAP_HD BcDecodeGeom bc_decode_geom(uint32_t width, uint32_t height, uint32_t row
     return g;
 }
 
-// grid = (bc_ctas, frames).  kBcRgtc1 alone writes the value to all of R,G,B with A=255.
+// grid = (bc_ctas, frames).  kBcRgtc1 alone writes the value to all of R,G,B with A=255.  kBcBc7 never merges alpha.
 template <int KIND>
 __global__ void __launch_bounds__(kBcThreads) bc_decode_kernel(const uint8_t *__restrict__ blocks,
                                                                 const uint8_t *__restrict__ alpha_blocks,
@@ -193,6 +198,9 @@ __global__ void __launch_bounds__(kBcThreads) bc_decode_kernel(const uint8_t *__
     } else if (KIND == kBcDxt1 || KIND == kBcRgtc1) {
         uint2 v = reinterpret_cast<const uint2 *>(in)[bi];
         decode_block(KIND, v.x, v.y, 0, 0, px);
+    } else if (KIND == kBcBc7) {
+        uint4 v = reinterpret_cast<const uint4 *>(in)[bi];
+        bc7_decode_block(v.x, v.y, v.z, v.w, px);
     } else {
         uint4 v = reinterpret_cast<const uint4 *>(in)[bi];
         decode_block(KIND, v.x, v.y, v.z, v.w, px);

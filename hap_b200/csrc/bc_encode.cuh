@@ -11,7 +11,8 @@
 
 namespace hapb200 {
 
-enum BcKind : int { kBcDxt1 = 0, kBcDxt5 = 1, kBcYCoCg = 2, kBcRgtc1 = 3, kBcYCoCgPlusAlpha = 4 };
+// kBcBc7 (BPTC RGBA UNORM, Hap R) is decoded only (bc7_decode.cuh): there is no BC7 block compressor
+enum BcKind : int { kBcDxt1 = 0, kBcDxt5 = 1, kBcYCoCg = 2, kBcRgtc1 = 3, kBcYCoCgPlusAlpha = 4, kBcBc7 = 5 };
 
 constexpr int kBcThreads = 128;
 #ifndef HAPB200_BC_MIN_BLOCKS

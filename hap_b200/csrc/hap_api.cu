@@ -270,9 +270,12 @@ bool codec_info(unsigned codec, CodecInfo &c)
     case HapB200Codec_HapY: c = {1, {HapFmt_YCoCg_DXT5, 0}, {16, 0}, kBcYCoCg}; return true;
     case HapB200Codec_HapM: c = {2, {HapFmt_YCoCg_DXT5, HapFmt_A_RGTC1}, {16, 8}, kBcYCoCgPlusAlpha}; return true;
     case HapB200Codec_HapA: c = {1, {HapFmt_A_RGTC1, 0}, {8, 0}, kBcRgtc1}; return true;
+    case HapB200Codec_Hap7: c = {1, {HapFmt_RGBA_BPTC_UNORM, 0}, {16, 0}, kBcBc7}; return true;
     default: return false;
     }
 }
+// the codecs the RGBA encode entry points take: every one with a block compressor (BC7 has none)
+bool codec_encodes(const CodecInfo &c) { return c.bc_kind != kBcBc7; }
 
 // hap.c:551-559 (SURVEY.md Q5): of two textures, one must be scaled YCoCg DXT5 or alpha RGTC1
 bool texture_formats_ok(unsigned count, const unsigned *f)
@@ -357,7 +360,8 @@ uint32_t launch_block_encode(const uint8_t *rgba, uint32_t frames, uint64_t fram
     case kBcDxt5: launch_bc_encode<kBcDxt5>(frames, st, rgba, g, blocks, refine); break;
     case kBcYCoCg: launch_bc_encode<kBcYCoCg>(frames, st, rgba, g, blocks, refine); break;
     case kBcRgtc1: launch_bc_encode<kBcRgtc1>(frames, st, rgba, g, blocks, refine); break;
-    default: launch_bc_encode<kBcYCoCgPlusAlpha>(frames, st, rgba, g, blocks, refine); break;
+    case kBcYCoCgPlusAlpha: launch_bc_encode<kBcYCoCgPlusAlpha>(frames, st, rgba, g, blocks, refine); break;
+    default: return HapResult_Bad_Arguments;   // kBcBc7: no block compressor (the entry points refuse it first)
     }
     return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
 }
@@ -382,7 +386,10 @@ uint32_t launch_block_decode(const uint8_t *blocks, const uint8_t *alpha, uint32
     case kBcDxt1: launch_bc_decode<kBcDxt1>(frames, st, blocks, alpha, g, rgba, frame_results); break;
     case kBcDxt5: launch_bc_decode<kBcDxt5>(frames, st, blocks, alpha, g, rgba, frame_results); break;
     case kBcRgtc1: launch_bc_decode<kBcRgtc1>(frames, st, blocks, alpha, g, rgba, frame_results); break;
-    default: launch_bc_decode<kBcYCoCg>(frames, st, blocks, alpha, g, rgba, frame_results); break;   // both scaled-YCoCg kinds
+    case kBcYCoCg:
+    case kBcYCoCgPlusAlpha: launch_bc_decode<kBcYCoCg>(frames, st, blocks, alpha, g, rgba, frame_results); break;
+    case kBcBc7: launch_bc_decode<kBcBc7>(frames, st, blocks, alpha, g, rgba, frame_results); break;
+    default: return HapResult_Internal_Error;
     }
     return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
 }
@@ -1017,8 +1024,8 @@ unsigned int HapB200BlockEncodeBatch(const void *rgba, unsigned int frames, unsi
                                      unsigned long blocksStride, void *stream)
 {
     CodecInfo ci;
-    if (!blocks || frames == 0 || !codec_info(codec, ci) || !rgba_geometry_ok(rgba, width, height, rowBytes, frameStride, true) ||
-        ((uintptr_t)blocks | blocksStride) % 16)
+    if (!blocks || frames == 0 || !codec_info(codec, ci) || !codec_encodes(ci) ||
+        !rgba_geometry_ok(rgba, width, height, rowBytes, frameStride, true) || ((uintptr_t)blocks | blocksStride) % 16)
         return HapResult_Bad_Arguments;
     HAP_ENTER(rgba, blocks);
     return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
@@ -1077,8 +1084,8 @@ unsigned int HapB200EncodeRGBABatch(const void *rgba, unsigned int frames, unsig
                                     void *stream)
 {
     CodecInfo ci;
-    if (!out || !used || frames == 0 || chunkCount == 0 || !codec_info(codec, ci) || !rgba_geometry_ok(rgba, width, height, rowBytes, frameStride, true) ||
-        (compressor != HapCompressorNone && compressor != HapCompressorSnappy))
+    if (!out || !used || frames == 0 || chunkCount == 0 || !codec_info(codec, ci) || !codec_encodes(ci) ||
+        !rgba_geometry_ok(rgba, width, height, rowBytes, frameStride, true) || (compressor != HapCompressorNone && compressor != HapCompressorSnappy))
         return HapResult_Bad_Arguments;
     if (outStride < HapB200MaxEncodedLengthRGBA(width, height, codec, chunkCount)) return HapResult_Buffer_Too_Small;
     HAP_ENTER(rgba, out);
@@ -1107,8 +1114,8 @@ unsigned int HapB200EncodeRGBA(const void *rgba, unsigned int width, unsigned in
                                unsigned long outputBufferBytes, unsigned long *outputBufferBytesUsed)
 {
     CodecInfo ci;
-    if (!outputBuffer || !outputBufferBytesUsed || chunkCount == 0 || !codec_info(codec, ci) || !rgba_geometry_ok(rgba, width, height, rowBytes, 0, false) ||
-        (compressor != HapCompressorNone && compressor != HapCompressorSnappy))
+    if (!outputBuffer || !outputBufferBytesUsed || chunkCount == 0 || !codec_info(codec, ci) || !codec_encodes(ci) ||
+        !rgba_geometry_ok(rgba, width, height, rowBytes, 0, false) || (compressor != HapCompressorNone && compressor != HapCompressorSnappy))
         return HapResult_Bad_Arguments;
     const unsigned long cap = HapB200MaxEncodedLengthRGBA(width, height, codec, chunkCount);
     if (outputBufferBytes < cap) return HapResult_Buffer_Too_Small;
@@ -1189,7 +1196,7 @@ unsigned int HapB200DecodeRGBA(const void *inputBuffer, unsigned long inputBuffe
         r = HapGetFrameTextureFormat(inputBuffer, inputBufferBytes, 1, &f1);
         if (r != HapResult_No_Error) return r;
     }
-    // the codec whose textures the frame has (BPTC frames carry no RGBA decoder here)
+    // the codec whose textures the frame has (BC6H frames, Hap HDR, have no RGBA decoder here: Bad_Frame)
     unsigned codec = 0;
     CodecInfo ci;
     while (codec_info(codec, ci) && (ci.textures != count || ci.fmt[0] != f0 || (count == 2 && ci.fmt[1] != f1))) codec++;

@@ -9,7 +9,8 @@ from .abi import HapABI
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 
-HapB200Codec_Hap1, HapB200Codec_Hap5, HapB200Codec_HapY, HapB200Codec_HapM, HapB200Codec_HapA = range(5)
+HapB200Codec_Hap1, HapB200Codec_Hap5, HapB200Codec_HapY, HapB200Codec_HapM, HapB200Codec_HapA, HapB200Codec_Hap7 = range(6)
+# HapB200Codec_Hap7 ("Hap R", BC7) decodes only: the RGBA encode entry points refuse it with HapResult_Bad_Arguments
 
 
 def library_path() -> str:

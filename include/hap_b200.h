@@ -23,8 +23,13 @@ enum HapB200Codec {
     HapB200Codec_Hap5 = 1, /* RGBA DXT5                        "Hap Alpha"      */
     HapB200Codec_HapY = 2, /* scaled YCoCg DXT5                "Hap Q"          */
     HapB200Codec_HapM = 3, /* scaled YCoCg DXT5 + alpha RGTC1  "Hap Q Alpha"    */
-    HapB200Codec_HapA = 4  /* alpha RGTC1                      "Hap Alpha-Only" */
+    HapB200Codec_HapA = 4, /* alpha RGTC1                      "Hap Alpha-Only" */
+    HapB200Codec_Hap7 = 5  /* RGBA BPTC (BC7) UNORM            "Hap R"          */
 };
+/* Hap R (Hap7) is decode-only: the library has no BC7 block compressor.  HapB200EncodeRGBA, HapB200EncodeRGBABatch and
+ * HapB200BlockEncodeBatch refuse it with HapResult_Bad_Arguments; HapEncode and HapB200EncodeBatch wrap BC7 textures that
+ * were compressed elsewhere.  The RGBA decoders turn BC7 blocks into RGBA8 exactly as the BPTC specification defines them,
+ * reserved blocks (first byte 0) included: those decode to (0, 0, 0, 0) in all 16 texels. */
 
 const char *HapB200Version(void);
 /* kernels launched by this library in this process so far (bench.py reports the delta) */
@@ -112,7 +117,8 @@ unsigned int HapB200EncodeRGBA(const void *rgba, unsigned int width, unsigned in
                                void *outputBuffer, unsigned long outputBufferBytes,
                                unsigned long *outputBufferBytesUsed);
 
-/* One Hap frame -> RGBA8 (all textures of the frame combined; YCoCg converted, alpha merged). */
+/* One Hap frame -> RGBA8 (all textures of the frame combined; YCoCg converted, alpha merged).  Every flavour but Hap HDR
+ * (BC6H) decodes; a frame of BC6H textures returns HapResult_Bad_Frame. */
 unsigned int HapB200DecodeRGBA(const void *inputBuffer, unsigned long inputBufferBytes, unsigned int width,
                                unsigned int height, void *rgba, unsigned long rowBytes);
 
@@ -147,7 +153,7 @@ unsigned int HapB200DecodeRGBABatch(const void *in, unsigned int frames, unsigne
                                     void *stream);
 
 /* Block codecs alone (K1-K4 / K8), batched: kind = HapB200Codec; HapM writes/reads the YCoCg plane at
- * blocks and the RGTC1 plane at blocks + HapB200TextureBytes(.., 0). */
+ * blocks and the RGTC1 plane at blocks + HapB200TextureBytes(.., 0).  Hap7 (BC7) decodes only. */
 unsigned int HapB200BlockEncodeBatch(const void *rgba, unsigned int frames, unsigned long frameStride,
                                      unsigned int width, unsigned int height, unsigned long rowBytes,
                                      unsigned int codec, void *blocks, unsigned long blocksStride, void *stream);

@@ -6,6 +6,7 @@
 // this library: without a CUDA device the compute entry points return HapResult_Internal_Error.
 #include "../../include/hap_b200.h"
 
+#include "bc6h_decode.cuh"
 #include "bc_decode.cuh"
 #include "bc_encode.cuh"
 #include "hap_assemble.cuh"
@@ -283,11 +284,13 @@ bool texture_formats_ok(unsigned count, const unsigned *f)
     return count != 2 || f[0] == HapFmt_YCoCg_DXT5 || f[1] == HapFmt_YCoCg_DXT5 || f[0] == HapFmt_A_RGTC1 || f[1] == HapFmt_A_RGTC1;
 }
 
-// width x height RGBA pictures, rows rowBytes apart.  aligned: the batch entry points' rules besides (16-byte aligned rows,
-// picture address and picture stride).  The block kernels hold the row pitch and the block index in 32 bits.
-bool rgba_geometry_ok(const void *rgba, unsigned width, unsigned height, unsigned long rowBytes, unsigned long frameStride, bool aligned)
+// width x height pictures of `bpp` bytes per pixel (4: RGBA8, 8: RGBA16F), rows rowBytes apart.  aligned: the batch entry
+// points' rules besides (16-byte aligned rows, picture address and picture stride).  The block kernels hold the row pitch and
+// the block index in 32 bits.
+bool rgba_geometry_ok(const void *rgba, unsigned width, unsigned height, unsigned long rowBytes, unsigned long frameStride, bool aligned,
+                      unsigned long bpp = 4)
 {
-    if (!rgba || width == 0 || height == 0 || width % 4 || height % 4 || rowBytes < 4ul * width) return false;
+    if (!rgba || width == 0 || height == 0 || width % 4 || height % 4 || rowBytes < bpp * width) return false;
     if (rowBytes > HAPB200_MAX_ROW_BYTES || (unsigned long)(width / 4) * (height / 4) > HAPB200_MAX_BLOCKS) return false;
     return !aligned || (rowBytes % 16 == 0 && ((uintptr_t)rgba | frameStride) % 16 == 0);
 }
@@ -390,6 +393,21 @@ uint32_t launch_block_decode(const uint8_t *blocks, const uint8_t *alpha, uint32
     case kBcYCoCgPlusAlpha: launch_bc_decode<kBcYCoCg>(frames, st, blocks, alpha, g, rgba, frame_results); break;
     case kBcBc7: launch_bc_decode<kBcBc7>(frames, st, blocks, alpha, g, rgba, frame_results); break;
     default: return HapResult_Internal_Error;
+    }
+    return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
+}
+
+// BC6H (Hap HDR) blocks -> RGBA16F.  Signedness per frame from frame_formats, or is_signed for all.  One launch per
+// kBcFramesPerLaunch frames.
+uint32_t launch_bc6h_decode(const uint8_t *blocks, uint32_t frames, uint64_t blocks_stride, uint32_t width, uint32_t height, uint8_t *rgba,
+                            uint64_t frame_stride, uint64_t row_bytes, cudaStream_t st, const uint32_t *frame_results,
+                            const uint32_t *frame_formats, bool is_signed)
+{
+    const BcDecodeGeom g = bc_decode_geom(width, height, (uint32_t)row_bytes, false, blocks_stride, 0, frame_stride);
+    for (uint32_t f0 = 0; f0 < frames; f0 += kBcFramesPerLaunch) {
+        const dim3 grid(bc_ctas(g.blocks_x, g.blocks_y), frames - f0 < kBcFramesPerLaunch ? frames - f0 : kBcFramesPerLaunch);
+        HAP_KLAUNCH(kStBcDecode, bc6h_decode_kernel, grid, dim3(kBcThreads), 0, st, blocks + f0 * g.in_stride, g, rgba + f0 * g.frame_bytes,
+                    frame_results ? frame_results + f0 : nullptr, frame_formats ? frame_formats + f0 : nullptr, is_signed ? 1u : 0u);
     }
     return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
 }
@@ -558,6 +576,40 @@ __global__ void ring_wait_kernel(const unsigned int *flag, unsigned int value, u
     }
 }
 }  // namespace
+
+// The single-frame picture decoders (HapB200DecodeRGBA, HapB200DecodeRGBAHalf): textures 0 .. count-1 of the frame, t[i]
+// bytes each, are decoded by HapDecode into device scratch (a texture that does not fill its room: Bad_Frame); then
+// launch(textures, picture, tight row bytes, stream) writes a tight picture of bpp bytes per pixel, which is copied to the
+// caller's rows.
+template <class Launch>
+uint32_t decode_frame_to_picture(const void *inputBuffer, unsigned long inputBufferBytes, unsigned count, const uint64_t t[2],
+                                 unsigned width, unsigned height, uint64_t bpp, void *picture, unsigned long rowBytes, Launch &&launch)
+{
+    HAP_ENTER(inputBuffer, picture);
+    const uint64_t tight = bpp * width;
+    // scratch from the device's stream-ordered pool on the legacy stream (the nested HapDecode calls below write it on
+    // that stream, or on a pooled stream they synchronise before returning): no cudaMalloc/cudaFree, no device-wide sync
+    DevBuf texb(kLegacyStream), imgb(kLegacyStream);
+    if (!texb.alloc(align16(t[0]) + align16(t[1]) + 16) || !imgb.alloc(tight * height)) { cudaGetLastError(); return HapResult_Internal_Error; }
+    if (cudaStreamSynchronize(kLegacyStream) != cudaSuccess) { cudaGetLastError(); return HapResult_Internal_Error; }   // the allocations are real now
+    auto serial = [](HapDecodeWorkFunction fn, void *p, unsigned n, void *) { for (unsigned i = 0; i < n; i++) fn(p, i); };
+    uint32_t r = HapResult_No_Error;
+    for (unsigned i = 0; i < count && r == HapResult_No_Error; i++) {
+        unsigned long used = 0;
+        unsigned fmt = 0;
+        r = HapDecode(inputBuffer, inputBufferBytes, i, serial, nullptr, texb.as<uint8_t>() + (i ? align16(t[0]) : 0), t[i], &used, &fmt);
+        if (r == HapResult_No_Error && used != t[i]) r = HapResult_Bad_Frame;
+    }
+    if (r == HapResult_No_Error) {
+        CallStream call(false);  // the scratch buffers are device memory filled on the legacy stream by HapDecode above
+        cudaStream_t st = call.st;
+        r = launch((const uint8_t *)texb.p, imgb.as<uint8_t>(), tight, st);
+        if (r == HapResult_No_Error &&
+            (cudaMemcpy2DAsync(picture, rowBytes, imgb.p, tight, tight, height, cudaMemcpyDefault, st) != cudaSuccess ||
+             cudaStreamSynchronize(st) != cudaSuccess)) { cudaGetLastError(); r = HapResult_Internal_Error; }
+    }
+    return r;
+}
 
 
 // =====================================================================================================
@@ -1196,39 +1248,79 @@ unsigned int HapB200DecodeRGBA(const void *inputBuffer, unsigned long inputBuffe
         r = HapGetFrameTextureFormat(inputBuffer, inputBufferBytes, 1, &f1);
         if (r != HapResult_No_Error) return r;
     }
-    // the codec whose textures the frame has (BC6H frames, Hap HDR, have no RGBA decoder here: Bad_Frame)
+    // the codec whose textures the frame has (BC6H frames, Hap HDR, decode to half floats: HapB200DecodeRGBAHalf; Bad_Frame here)
     unsigned codec = 0;
     CodecInfo ci;
     while (codec_info(codec, ci) && (ci.textures != count || ci.fmt[0] != f0 || (count == 2 && ci.fmt[1] != f1))) codec++;
     if (!codec_info(codec, ci)) return HapResult_Bad_Frame;
-    HAP_ENTER(inputBuffer, rgba);
-    const uint64_t t0 = HapB200TextureBytes(width, height, codec, 0), t1 = HapB200TextureBytes(width, height, codec, 1);
-    const uint64_t tight = 4ull * width;
-    // scratch from the device's stream-ordered pool on the legacy stream (the nested HapDecode calls below write it on
-    // that stream, or on a pooled stream they synchronise before returning): no cudaMalloc/cudaFree, no device-wide sync
-    DevBuf dxtb(kLegacyStream), imgb(kLegacyStream);
-    if (!dxtb.alloc(align16(t0) + align16(t1) + 16) || !imgb.alloc(tight * height)) { cudaGetLastError(); return HapResult_Internal_Error; }
-    void *dxt = dxtb.p, *img = imgb.p;
-    if (cudaStreamSynchronize(kLegacyStream) != cudaSuccess) { cudaGetLastError(); return HapResult_Internal_Error; }   // the allocations are real now
-    auto serial = [](HapDecodeWorkFunction fn, void *p, unsigned n, void *) { for (unsigned i = 0; i < n; i++) fn(p, i); };
-    unsigned long used = 0;
-    unsigned fmt = 0;
-    r = HapDecode(inputBuffer, inputBufferBytes, 0, serial, nullptr, dxt, t0, &used, &fmt);
-    if (r == HapResult_No_Error && used != t0) r = HapResult_Bad_Frame;
-    if (r == HapResult_No_Error && count == 2) {
-        r = HapDecode(inputBuffer, inputBufferBytes, 1, serial, nullptr, (uint8_t *)dxt + align16(t0), t1, &used, &fmt);
-        if (r == HapResult_No_Error && used != t1) r = HapResult_Bad_Frame;
-    }
-    if (r == HapResult_No_Error) {
-        CallStream call(false);  // dxt / img are device buffers filled on the legacy stream by HapDecode above
-        cudaStream_t st = call.st;
-        r = launch_block_decode((const uint8_t *)dxt, (const uint8_t *)dxt + align16(t0), 1, 0, 0, width, height, ci, (uint8_t *)img,
-                                0, tight, st);
-        if (r == HapResult_No_Error &&
-            (cudaMemcpy2DAsync(rgba, rowBytes, img, tight, tight, height, cudaMemcpyDefault, st) != cudaSuccess ||
-             cudaStreamSynchronize(st) != cudaSuccess)) { cudaGetLastError(); r = HapResult_Internal_Error; }
-    }
-    return r;
+    const uint64_t t[2] = {HapB200TextureBytes(width, height, codec, 0), HapB200TextureBytes(width, height, codec, 1)};
+    return decode_frame_to_picture(inputBuffer, inputBufferBytes, count, t, width, height, 4, rgba, rowBytes,
+                                   [&](const uint8_t *tex, uint8_t *img, uint64_t tight, cudaStream_t st) {
+                                       return launch_block_decode(tex, tex + align16(t[0]), 1, 0, 0, width, height, ci, img, 0, tight, st);
+                                   });
+}
+
+bool is_bc6h_format(unsigned f) { return f == HapFmt_RGB_BPTC_UFLOAT || f == HapFmt_RGB_BPTC_SFLOAT; }
+
+unsigned int HapB200BlockDecodeHalfBatch(const void *blocks, unsigned int frames, unsigned long blocksStride, unsigned int width,
+                                         unsigned int height, unsigned int textureFormat, void *rgbaHalf, unsigned long frameStride,
+                                         unsigned long rowBytes, void *stream)
+{
+    if (!blocks || frames == 0 || !is_bc6h_format(textureFormat) || !rgba_geometry_ok(rgbaHalf, width, height, rowBytes, frameStride, true, 8) ||
+        ((uintptr_t)blocks | blocksStride) % 16)
+        return HapResult_Bad_Arguments;
+    HAP_ENTER(blocks, rgbaHalf);
+    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
+        return launch_bc6h_decode((const uint8_t *)blocks, frames, blocksStride, width, height, (uint8_t *)rgbaHalf, frameStride, rowBytes, st,
+                                  nullptr, nullptr, textureFormat == HapFmt_RGB_BPTC_SFLOAT);
+    });
+}
+
+unsigned int HapB200DecodeRGBAHalfBatch(const void *in, unsigned int frames, unsigned long inStride, const unsigned long long *inBytes,
+                                        unsigned int maxChunks, unsigned int width, unsigned int height, void *rgbaHalf,
+                                        unsigned long frameStride, unsigned long rowBytes, unsigned int *results, void *stream)
+{
+    if (!in || !inBytes || !results || frames == 0 || maxChunks == 0 || !rgba_geometry_ok(rgbaHalf, width, height, rowBytes, frameStride, true, 8))
+        return HapResult_Bad_Arguments;
+    HAP_ENTER(in, rgbaHalf);
+    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
+        const uint64_t t0 = (uint64_t)(width / 4) * (height / 4) * 16, stride = align16(t0);
+        DevBuf tex(st), used(st), formats(st);
+        if (!tex.alloc(stride * frames + 16) || !used.alloc(8ull * frames) || !formats.alloc(4ull * frames)) {
+            cudaGetLastError();
+            return HapResult_Internal_Error;
+        }
+        // texture 0 of every frame, offered exactly its BC6H size; then a frame that is not one BC6H texture of that size
+        // reports Bad_Frame, other failures keep the decoder's code, and failed frames are zeroed
+        const uint32_t r = launch_decode_batch((const uint8_t *)in, frames, inStride, inBytes, 0, maxChunks, tex.as<uint8_t>(), stride, t0,
+                                               used.as<unsigned long long>(), formats.as<uint32_t>(), results, st);
+        if (r != HapResult_No_Error) return r;
+        HAP_KLAUNCH(kStCollect, hap_check_bc6h_frames_kernel, dim3((frames + 127) / 128), dim3(128), 0, st, (const uint8_t *)in, (uint64_t)inStride,
+                    inBytes, frames, used.as<unsigned long long>(), formats.as<uint32_t>(), (unsigned long long)t0, results);
+        return launch_bc6h_decode(tex.as<uint8_t>(), frames, stride, width, height, (uint8_t *)rgbaHalf, frameStride, rowBytes, st, results,
+                                  formats.as<uint32_t>(), false);
+    });
+}
+
+unsigned int HapB200DecodeRGBAHalf(const void *inputBuffer, unsigned long inputBufferBytes, unsigned int width, unsigned int height,
+                                   void *rgbaHalf, unsigned long rowBytes)
+{
+    if (!inputBuffer || !rgba_geometry_ok(rgbaHalf, width, height, rowBytes, 0, false, 8)) return HapResult_Bad_Arguments;
+    unsigned count = 0, fmt = 0;
+    uint32_t r = HapGetFrameTextureCount(inputBuffer, inputBufferBytes, &count);
+    if (r != HapResult_No_Error) return r;
+    r = HapGetFrameTextureFormat(inputBuffer, inputBufferBytes, 0, &fmt);
+    if (r != HapResult_No_Error) return r;
+    if (count != 1 || !is_bc6h_format(fmt)) return HapResult_Bad_Frame;
+    const uint64_t t[2] = {(uint64_t)(width / 4) * (height / 4) * 16, 0};
+    r = decode_frame_to_picture(inputBuffer, inputBufferBytes, 1, t, width, height, 8, rgbaHalf, rowBytes,
+                                [&](const uint8_t *tex, uint8_t *img, uint64_t tight, cudaStream_t st) {
+                                    return launch_bc6h_decode(tex, 1, 0, width, height, img, 0, tight, st, nullptr, nullptr,
+                                                              fmt == HapFmt_RGB_BPTC_SFLOAT);
+                                });
+    // the room offered is the picture's texture size: a texture too large for it (HapDecode: Buffer_Too_Small) is not this
+    // picture's texture either
+    return r == HapResult_Buffer_Too_Small ? (uint32_t)HapResult_Bad_Frame : r;
 }
 
 // ---- include/hap_mov.h: QuickTime sample tables around Hap frames (host code only) -------------------------

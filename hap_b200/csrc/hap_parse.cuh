@@ -163,4 +163,27 @@ __global__ void hap_check_texture_kernel(uint32_t frames, const unsigned long lo
     else if (merged[f] == HapResult_No_Error) merged[f] = r;
 }
 
+// RGBA16F decode path (Hap HDR): texture 0 of every frame was decoded into room of exactly want_bytes.  A frame must be
+// one BC6H texture of that size: a texture larger than the room (the prepass's Buffer_Too_Small: capacity is the only
+// limit the batch prepass sets), of another size or format, or a frame that has a texture 1 reports Bad_Frame.  Other
+// failures keep their code.
+__global__ void hap_check_bc6h_frames_kernel(const uint8_t *__restrict__ in, uint64_t in_stride,
+                                             const unsigned long long *__restrict__ in_bytes, uint32_t frames,
+                                             const unsigned long long *__restrict__ used, const uint32_t *__restrict__ formats,
+                                             unsigned long long want_bytes, uint32_t *results)
+{
+    const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= frames) return;
+    uint32_t r = results[f];
+    if (r == HapResult_Buffer_Too_Small) {
+        r = HapResult_Bad_Frame;
+    } else if (r == HapResult_No_Error) {
+        Located second;
+        const bool bc6h = formats[f] == HapFmt_RGB_BPTC_UFLOAT || formats[f] == HapFmt_RGB_BPTC_SFLOAT;
+        if (!bc6h || used[f] != want_bytes || locate_texture(in + (uint64_t)f * in_stride, (uint32_t)in_bytes[f], 1, second) == HapResult_No_Error)
+            r = HapResult_Bad_Frame;
+    }
+    results[f] = r;
+}
+
 }  // namespace hapb200

@@ -57,6 +57,12 @@ class HapB200(HapABI):
         L.HapB200BlockEncodeBatch.argtypes = [vp, u, ul, u, u, ul, u, vp, ul, vp]
         L.HapB200BlockDecodeBatch.restype = u
         L.HapB200BlockDecodeBatch.argtypes = [vp, u, ul, u, u, u, vp, ul, ul, vp]
+        L.HapB200DecodeRGBAHalf.restype = u
+        L.HapB200DecodeRGBAHalf.argtypes = [vp, ul, u, u, vp, ul]
+        L.HapB200DecodeRGBAHalfBatch.restype = u
+        L.HapB200DecodeRGBAHalfBatch.argtypes = [vp, u, ul, vp, u, u, u, vp, ul, ul, vp, vp]
+        L.HapB200BlockDecodeHalfBatch.restype = u
+        L.HapB200BlockDecodeHalfBatch.argtypes = [vp, u, ul, u, u, u, vp, ul, ul, vp]
         for name, args in (("RingCreate", [C.c_int, ul, C.POINTER(vp), vp]), ("RingDestroy", [C.c_int, vp]),
                            ("RingOpen", [C.c_int, vp, C.POINTER(vp)]), ("RingClose", [C.c_int, vp]),
                            ("RingAttach", [C.c_int, C.c_int]), ("RingPublish", [C.c_int, vp, u, vp]), ("RingWait", [C.c_int, vp, u, u, vp])):
@@ -171,6 +177,30 @@ class HapB200(HapABI):
     def block_decode_batch(self, blocks, frames, blocks_stride, w, h, codec, rgba, frame_stride, row_bytes=None, stream=None):
         return int(self.lib.HapB200BlockDecodeBatch(blocks, frames, blocks_stride, w, h, codec, rgba, frame_stride,
                                                     row_bytes or 4 * w, stream))
+
+    # -- Hap HDR (BC6H) -> RGBA16F: 8 bytes per pixel, binary16 R, G, B, A (A = 1.0) ---------------------------------------
+    def decode_rgba_half(self, frame, w, h, out=None, row_bytes=None, frame_bytes=None):
+        """One Hap HDR frame (buffer object or (addr, nbytes)) -> (result, RGBA16F bytes when `out` is not given)"""
+        from .abi import _as_ptr
+        faddr, fn = _as_ptr(frame)
+        if frame_bytes is not None:
+            fn = frame_bytes
+        own = out is None
+        if own:
+            out = bytearray(8 * w * h)
+        oaddr, _ = _as_ptr(out)
+        r = self.lib.HapB200DecodeRGBAHalf(faddr, fn, w, h, oaddr, row_bytes or 8 * w)
+        return int(r), (bytes(out) if own and r == 0 else None)
+
+    def decode_rgba_half_batch(self, frames_ptr, frames, in_stride, in_bytes, max_chunks, w, h, rgba, frame_stride, results,
+                               row_bytes=None, stream=None):
+        return int(self.lib.HapB200DecodeRGBAHalfBatch(frames_ptr, frames, in_stride, in_bytes, max_chunks, w, h, rgba,
+                                                       frame_stride, row_bytes or 8 * w, results, stream))
+
+    def block_decode_half_batch(self, blocks, frames, blocks_stride, w, h, texture_format, rgba, frame_stride, row_bytes=None,
+                                stream=None):
+        return int(self.lib.HapB200BlockDecodeHalfBatch(blocks, frames, blocks_stride, w, h, texture_format, rgba, frame_stride,
+                                                        row_bytes or 8 * w, stream))
 
 
     # -- delivery rings (include/hap_b200.h): frames written straight into another GPU's memory -----------------

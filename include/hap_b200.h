@@ -117,8 +117,8 @@ unsigned int HapB200EncodeRGBA(const void *rgba, unsigned int width, unsigned in
                                void *outputBuffer, unsigned long outputBufferBytes,
                                unsigned long *outputBufferBytesUsed);
 
-/* One Hap frame -> RGBA8 (all textures of the frame combined; YCoCg converted, alpha merged).  Every flavour but Hap HDR
- * (BC6H) decodes; a frame of BC6H textures returns HapResult_Bad_Frame. */
+/* One Hap frame -> RGBA8 (all textures of the frame combined; YCoCg converted, alpha merged).  Hap HDR (BC6H) frames
+ * decode to half floats instead (HapB200DecodeRGBAHalf below); here they return HapResult_Bad_Frame. */
 unsigned int HapB200DecodeRGBA(const void *inputBuffer, unsigned long inputBufferBytes, unsigned int width,
                                unsigned int height, void *rgba, unsigned long rowBytes);
 
@@ -153,13 +153,42 @@ unsigned int HapB200DecodeRGBABatch(const void *in, unsigned int frames, unsigne
                                     void *stream);
 
 /* Block codecs alone (K1-K4 / K8), batched: kind = HapB200Codec; HapM writes/reads the YCoCg plane at
- * blocks and the RGTC1 plane at blocks + HapB200TextureBytes(.., 0).  Hap7 (BC7) decodes only. */
+ * blocks and the RGTC1 plane at blocks + HapB200TextureBytes(.., 0).  Hap7 (BC7) decodes only.  BC6H blocks: see
+ * HapB200BlockDecodeHalfBatch. */
 unsigned int HapB200BlockEncodeBatch(const void *rgba, unsigned int frames, unsigned long frameStride,
                                      unsigned int width, unsigned int height, unsigned long rowBytes,
                                      unsigned int codec, void *blocks, unsigned long blocksStride, void *stream);
 unsigned int HapB200BlockDecodeBatch(const void *blocks, unsigned int frames, unsigned long blocksStride,
                                      unsigned int width, unsigned int height, unsigned int codec, void *rgba,
                                      unsigned long frameStride, unsigned long rowBytes, void *stream);
+
+/* ---- Hap HDR (BC6H, "HapH") -> RGBA16F ---------------------------------------------------------------------------------
+ * BC6H decodes to half floats: every pixel is 8 bytes, four IEEE binary16 values R, G, B, A, with A = 1.0 (0x3C00).
+ * Blocks decode exactly as the BPTC specification defines them, UF16 (HapTextureFormat_RGB_BPTC_UNSIGNED_FLOAT) or SF16
+ * (HapTextureFormat_RGB_BPTC_SIGNED_FLOAT), interpolation rounding (+32) included.  Every output is finite: an SF16
+ * endpoint of -32768 (mode 14) is taken as -32767, whose scaled magnitude is the largest finite half.  A negative value
+ * whose magnitude scales to 0 is written as +0 (0x0000), as the specification's integer form gives it.  The four reserved
+ * mode values decode to (0, 0, 0, 1.0).  Geometry as for the RGBA8 entry points with 8 bytes per pixel: width and height
+ * multiples of 4, 8 * width <= rowBytes <= HAPB200_MAX_ROW_BYTES, at most HAPB200_MAX_BLOCKS blocks; the batch entry points
+ * take device pointers, 16-byte aligned rows, pictures and strides, and any number of frames. */
+
+/* One Hap HDR frame (host or device pointers) -> RGBA16F.  A frame that is not one BC6H texture of exactly
+ * (width/4)*(height/4)*16 bytes returns HapResult_Bad_Frame. */
+unsigned int HapB200DecodeRGBAHalf(const void *inputBuffer, unsigned long inputBufferBytes, unsigned int width,
+                                   unsigned int height, void *rgbaHalf, unsigned long rowBytes);
+/* HapB200DecodeRGBABatch for Hap HDR: each frame decodes as its own texture says (UF16 or SF16).  A frame that is not one
+ * BC6H texture of exactly (width/4)*(height/4)*16 bytes (another format, a larger or smaller texture, a second texture)
+ * reports Bad_Frame in results[f], as HapB200DecodeRGBAHalf answers for it; other failures keep the chunk decoder's code;
+ * the picture of a failed frame is all zero bytes. */
+unsigned int HapB200DecodeRGBAHalfBatch(const void *in, unsigned int frames, unsigned long inStride,
+                                        const unsigned long long *inBytes, unsigned int maxChunks, unsigned int width,
+                                        unsigned int height, void *rgbaHalf, unsigned long frameStride,
+                                        unsigned long rowBytes, unsigned int *results, void *stream);
+/* HapB200BlockDecodeBatch for BC6H blocks: textureFormat = HapTextureFormat_RGB_BPTC_UNSIGNED_FLOAT or
+ * HapTextureFormat_RGB_BPTC_SIGNED_FLOAT (anything else: HapResult_Bad_Arguments). */
+unsigned int HapB200BlockDecodeHalfBatch(const void *blocks, unsigned int frames, unsigned long blocksStride,
+                                         unsigned int width, unsigned int height, unsigned int textureFormat,
+                                         void *rgbaHalf, unsigned long frameStride, unsigned long rowBytes, void *stream);
 
 #ifdef __cplusplus
 }

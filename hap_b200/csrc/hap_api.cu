@@ -7,6 +7,7 @@
 #include "../../include/hap_b200.h"
 
 #include "bc6h_decode.cuh"
+#include "bc6h_encode.cuh"
 #include "bc_decode.cuh"
 #include "bc_encode.cuh"
 #include "hap_assemble.cuh"
@@ -367,6 +368,43 @@ uint32_t launch_block_encode(const uint8_t *rgba, uint32_t frames, uint64_t fram
     default: return HapResult_Bad_Arguments;   // kBcBc7: no block compressor (the entry points refuse it first)
     }
     return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
+}
+
+// RGBA16F pictures -> BC6H blocks (Hap HDR), SF16 when is_signed, else UF16.  One launch per kBcFramesPerLaunch frames.
+uint32_t launch_bc6h_encode(const uint8_t *rgba, uint32_t frames, uint64_t frame_stride, uint32_t width, uint32_t height, uint64_t row_bytes,
+                            uint8_t *blocks, uint64_t blocks_stride, bool is_signed, cudaStream_t st)
+{
+    const BcGeom g = bc_encode_geom(width, height, (uint32_t)row_bytes, frame_stride, blocks_stride, 0);   // (rgba_geometry_ok: row_bytes < 2^32)
+    for (uint32_t f0 = 0; f0 < frames; f0 += kBcFramesPerLaunch) {
+        const dim3 grid(bc_ctas(g.blocks_x, g.blocks_y), frames - f0 < kBcFramesPerLaunch ? frames - f0 : kBcFramesPerLaunch);
+        HAP_KLAUNCH(kStBcEncode, bc6h_encode_kernel, grid, dim3(kBcThreads), 0, st, rgba + f0 * g.frame_bytes, g, blocks + f0 * g.out_stride,
+                    is_signed ? 1u : 0u);
+    }
+    return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
+}
+
+// The tail of the picture batch encoders: encode_blocks(textures, stride) fills the textures of every frame into device
+// scratch (frame f at textures + f*stride, texture 1 at align16(t[0]) inside it), then the frames are laid out from them at
+// out + f*out_stride, lengths in used[f].
+template <class EncodeBlocks>
+uint32_t encode_frames_from_blocks(uint32_t frames, uint32_t count, const uint64_t t[2], const uint32_t fmt[2], unsigned compressor,
+                                   unsigned chunk_count, uint8_t *out, uint64_t out_stride, unsigned long long *used, cudaStream_t st,
+                                   EncodeBlocks &&encode_blocks)
+{
+    const uint64_t stride = align16(t[0]) + align16(t[1]);
+    DevBuf tex(st);
+    if (!tex.alloc(stride * frames + 16)) { cudaGetLastError(); return (uint32_t)HapResult_Internal_Error; }
+    uint32_t r = encode_blocks(tex.as<uint8_t>(), stride);
+    if (r != HapResult_No_Error) return r;
+    TextureArgs ta[2] = {{t[0], fmt[0], compressor, chunk_count}, {t[1], fmt[1], compressor, chunk_count}};
+    FrameGeom G;
+    r = build_frame_geom(count, ta, G);
+    if (r != HapResult_No_Error) return r;
+    for (unsigned i = 0; i < count; i++) {
+        G.s[i].in_offset = i ? align16(t[0]) : 0;
+        G.s[i].in_stride = stride;
+    }
+    return launch_encode(tex.as<uint8_t>(), G, frames, out, out_stride, used, st);
 }
 
 template <int KIND>
@@ -1142,22 +1180,12 @@ unsigned int HapB200EncodeRGBABatch(const void *rgba, unsigned int frames, unsig
     if (outStride < HapB200MaxEncodedLengthRGBA(width, height, codec, chunkCount)) return HapResult_Buffer_Too_Small;
     HAP_ENTER(rgba, out);
     return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
-        const uint64_t t0 = HapB200TextureBytes(width, height, codec, 0), t1 = HapB200TextureBytes(width, height, codec, 1);
-        const uint64_t dxt_stride = align16(t0) + align16(t1);
-        DevBuf dxt(st);
-        if (!dxt.alloc(dxt_stride * frames + 16)) { cudaGetLastError(); return (uint32_t)HapResult_Internal_Error; }
-        uint32_t r = launch_block_encode((const uint8_t *)rgba, frames, frameStride, width, height, rowBytes, ci, dxt.as<uint8_t>(),
-                                         dxt_stride, align16(t0), st);
-        if (r != HapResult_No_Error) return r;
-        TextureArgs ta[2] = {{t0, ci.fmt[0], compressor, chunkCount}, {t1, ci.fmt[1], compressor, chunkCount}};
-        FrameGeom G;
-        r = build_frame_geom(ci.textures, ta, G);
-        if (r != HapResult_No_Error) return r;
-        for (unsigned i = 0; i < ci.textures; i++) {
-            G.s[i].in_offset = i ? align16(t0) : 0;
-            G.s[i].in_stride = dxt_stride;
-        }
-        return launch_encode(dxt.as<uint8_t>(), G, frames, (uint8_t *)out, outStride, used, st);
+        const uint64_t t[2] = {HapB200TextureBytes(width, height, codec, 0), HapB200TextureBytes(width, height, codec, 1)};
+        return encode_frames_from_blocks(frames, ci.textures, t, ci.fmt, compressor, chunkCount, (uint8_t *)out, outStride, used, st,
+                                         [&](uint8_t *tex, uint64_t stride) {
+                                             return launch_block_encode((const uint8_t *)rgba, frames, frameStride, width, height, rowBytes, ci,
+                                                                        tex, stride, align16(t[0]), st);
+                                         });
     });
 }
 
@@ -1321,6 +1349,78 @@ unsigned int HapB200DecodeRGBAHalf(const void *inputBuffer, unsigned long inputB
     // the room offered is the picture's texture size: a texture too large for it (HapDecode: Buffer_Too_Small) is not this
     // picture's texture either
     return r == HapResult_Buffer_Too_Small ? (uint32_t)HapResult_Bad_Frame : r;
+}
+
+// ---- Hap HDR encoding: RGBA16F -> BC6H (bc6h_encode.cuh) ----
+
+// HapMaxEncodedLength of the one BC6H texture of a width x height picture
+static unsigned long bc6h_max_encoded_length(unsigned width, unsigned height, unsigned textureFormat, unsigned chunkCount)
+{
+    unsigned long len = (unsigned long)(width / 4) * (height / 4) * 16;
+    unsigned fmt = textureFormat, chunks = chunkCount;
+    return HapMaxEncodedLength(1, &len, &fmt, &chunks);
+}
+
+unsigned int HapB200BlockEncodeHalfBatch(const void *rgbaHalf, unsigned int frames, unsigned long frameStride, unsigned int width,
+                                         unsigned int height, unsigned long rowBytes, unsigned int textureFormat, void *blocks,
+                                         unsigned long blocksStride, void *stream)
+{
+    if (!blocks || frames == 0 || !is_bc6h_format(textureFormat) || !rgba_geometry_ok(rgbaHalf, width, height, rowBytes, frameStride, true, 8) ||
+        ((uintptr_t)blocks | blocksStride) % 16)
+        return HapResult_Bad_Arguments;
+    HAP_ENTER(rgbaHalf, blocks);
+    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
+        return launch_bc6h_encode((const uint8_t *)rgbaHalf, frames, frameStride, width, height, rowBytes, (uint8_t *)blocks, blocksStride,
+                                  textureFormat == HapFmt_RGB_BPTC_SFLOAT, st);
+    });
+}
+
+unsigned int HapB200EncodeRGBAHalfBatch(const void *rgbaHalf, unsigned int frames, unsigned long frameStride, unsigned int width,
+                                        unsigned int height, unsigned long rowBytes, unsigned int textureFormat, unsigned int compressor,
+                                        unsigned int chunkCount, void *out, unsigned long outStride, unsigned long long *used, void *stream)
+{
+    if (!out || !used || frames == 0 || chunkCount == 0 || !is_bc6h_format(textureFormat) ||
+        !rgba_geometry_ok(rgbaHalf, width, height, rowBytes, frameStride, true, 8) || ((uintptr_t)out | outStride) % 16 ||
+        (compressor != HapCompressorNone && compressor != HapCompressorSnappy))
+        return HapResult_Bad_Arguments;
+    if (outStride < bc6h_max_encoded_length(width, height, textureFormat, chunkCount)) return HapResult_Buffer_Too_Small;
+    HAP_ENTER(rgbaHalf, out);
+    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
+        const uint64_t t[2] = {(uint64_t)(width / 4) * (height / 4) * 16, 0};
+        const uint32_t fmt[2] = {textureFormat, 0};
+        return encode_frames_from_blocks(frames, 1, t, fmt, compressor, chunkCount, (uint8_t *)out, outStride, used, st,
+                                         [&](uint8_t *tex, uint64_t stride) {
+                                             return launch_bc6h_encode((const uint8_t *)rgbaHalf, frames, frameStride, width, height, rowBytes,
+                                                                       tex, stride, textureFormat == HapFmt_RGB_BPTC_SFLOAT, st);
+                                         });
+    });
+}
+
+unsigned int HapB200EncodeRGBAHalf(const void *rgbaHalf, unsigned int width, unsigned int height, unsigned long rowBytes,
+                                   unsigned int textureFormat, unsigned int compressor, unsigned int chunkCount, void *outputBuffer,
+                                   unsigned long outputBufferBytes, unsigned long *outputBufferBytesUsed)
+{
+    if (!outputBuffer || !outputBufferBytesUsed || chunkCount == 0 || !is_bc6h_format(textureFormat) ||
+        !rgba_geometry_ok(rgbaHalf, width, height, rowBytes, 0, false, 8) || (compressor != HapCompressorNone && compressor != HapCompressorSnappy))
+        return HapResult_Bad_Arguments;
+    const unsigned long cap = bc6h_max_encoded_length(width, height, textureFormat, chunkCount);
+    if (outputBufferBytes < cap) return HapResult_Buffer_Too_Small;
+    HAP_ENTER(rgbaHalf, outputBuffer);
+    CallStream call(!is_device(rgbaHalf) && !is_device(outputBuffer));
+    cudaStream_t st = call.st;
+    DevBuf img(st), frame(st), used(st);
+    const uint64_t tight = 8ull * width;
+    if (!img.alloc(tight * height) || !frame.alloc(align16(cap)) || !used.alloc(32)) { cudaGetLastError(); return HapResult_Internal_Error; }
+    if (cudaMemcpy2DAsync(img.p, tight, rgbaHalf, rowBytes, tight, height, cudaMemcpyDefault, st) != cudaSuccess) { cudaGetLastError(); return HapResult_Internal_Error; }
+    uint32_t r = HapB200EncodeRGBAHalfBatch(img.p, 1, align16(tight * height), width, height, tight, textureFormat, compressor, chunkCount,
+                                            frame.p, align16(cap), used.as<unsigned long long>(), st);
+    if (r != HapResult_No_Error) return r;
+    unsigned long long total = 0;
+    if (cudaMemcpyAsync(&total, used.p, sizeof total, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess ||
+        total > outputBufferBytes || cudaMemcpyAsync(outputBuffer, frame.p, total, cudaMemcpyDefault, st) != cudaSuccess ||
+        cudaStreamSynchronize(st) != cudaSuccess) { cudaGetLastError(); return HapResult_Internal_Error; }
+    *outputBufferBytesUsed = (unsigned long)total;
+    return HapResult_No_Error;
 }
 
 // ---- include/hap_mov.h: QuickTime sample tables around Hap frames (host code only) -------------------------

@@ -63,6 +63,12 @@ class HapB200(HapABI):
         L.HapB200DecodeRGBAHalfBatch.argtypes = [vp, u, ul, vp, u, u, u, vp, ul, ul, vp, vp]
         L.HapB200BlockDecodeHalfBatch.restype = u
         L.HapB200BlockDecodeHalfBatch.argtypes = [vp, u, ul, u, u, u, vp, ul, ul, vp]
+        L.HapB200EncodeRGBAHalf.restype = u
+        L.HapB200EncodeRGBAHalf.argtypes = [vp, u, u, ul, u, u, u, vp, ul, C.POINTER(ul)]
+        L.HapB200EncodeRGBAHalfBatch.restype = u
+        L.HapB200EncodeRGBAHalfBatch.argtypes = [vp, u, ul, u, u, ul, u, u, u, vp, ul, vp, vp]
+        L.HapB200BlockEncodeHalfBatch.restype = u
+        L.HapB200BlockEncodeHalfBatch.argtypes = [vp, u, ul, u, u, ul, u, vp, ul, vp]
         for name, args in (("RingCreate", [C.c_int, ul, C.POINTER(vp), vp]), ("RingDestroy", [C.c_int, vp]),
                            ("RingOpen", [C.c_int, vp, C.POINTER(vp)]), ("RingClose", [C.c_int, vp]),
                            ("RingAttach", [C.c_int, C.c_int]), ("RingPublish", [C.c_int, vp, u, vp]), ("RingWait", [C.c_int, vp, u, u, vp])):
@@ -201,6 +207,36 @@ class HapB200(HapABI):
                                 stream=None):
         return int(self.lib.HapB200BlockDecodeHalfBatch(blocks, frames, blocks_stride, w, h, texture_format, rgba, frame_stride,
                                                         row_bytes or 8 * w, stream))
+
+    # -- RGBA16F -> Hap HDR (BC6H): texture_format UF16 or SF16; A is ignored --------------------------------------------------
+    def max_encoded_length_half(self, w, h, texture_format, chunks) -> int:
+        """the output a frame of encode_rgba_half / encode_rgba_half_batch needs (HapMaxEncodedLength of its one texture)"""
+        return self.max_encoded_length([(w // 4) * (h // 4) * 16], [texture_format], [chunks])
+
+    def encode_rgba_half(self, rgba, w, h, texture_format, compressor=1, chunks=1, row_bytes=None, out=None, out_capacity=None):
+        """rgba: buffer object or (addr, nbytes), 8 bytes per pixel.  Returns (result, frame bytes | used)."""
+        from .abi import _as_ptr
+        addr, _ = _as_ptr(rgba)
+        cap = self.max_encoded_length_half(w, h, texture_format, chunks) if out_capacity is None else out_capacity
+        own = out is None
+        if own:
+            out = bytearray(max(cap, 1))
+        oaddr, _ = _as_ptr(out)
+        used = C.c_ulong(0)
+        r = self.lib.HapB200EncodeRGBAHalf(addr, w, h, row_bytes or 8 * w, texture_format, compressor, chunks, oaddr, cap, C.byref(used))
+        if r != 0:
+            return int(r), None
+        return 0, (bytes(memoryview(out)[: used.value]) if own else used.value)
+
+    def encode_rgba_half_batch(self, rgba, frames, frame_stride, w, h, texture_format, compressor, chunks, out, out_stride, used,
+                               row_bytes=None, stream=None):
+        return int(self.lib.HapB200EncodeRGBAHalfBatch(rgba, frames, frame_stride, w, h, row_bytes or 8 * w, texture_format,
+                                                       compressor, chunks, out, out_stride, used, stream))
+
+    def block_encode_half_batch(self, rgba, frames, frame_stride, w, h, texture_format, blocks, blocks_stride, row_bytes=None,
+                                stream=None):
+        return int(self.lib.HapB200BlockEncodeHalfBatch(rgba, frames, frame_stride, w, h, row_bytes or 8 * w, texture_format,
+                                                        blocks, blocks_stride, stream))
 
 
     # -- delivery rings (include/hap_b200.h): frames written straight into another GPU's memory -----------------

@@ -190,6 +190,37 @@ unsigned int HapB200BlockDecodeHalfBatch(const void *blocks, unsigned int frames
                                          unsigned int width, unsigned int height, unsigned int textureFormat,
                                          void *rgbaHalf, unsigned long frameStride, unsigned long rowBytes, void *stream);
 
+/* ---- Hap HDR (BC6H, "HapH") <- RGBA16F --------------------------------------------------------------------------------
+ * The encoders take RGBA16F pictures (8 bytes per pixel, binary16 R, G, B, A; A is ignored) and write BC6H blocks of
+ * textureFormat = HapTextureFormat_RGB_BPTC_UNSIGNED_FLOAT (UF16) or HapTextureFormat_RGB_BPTC_SIGNED_FLOAT (SF16);
+ * anything else is refused with HapResult_Bad_Arguments.  A frame holds one BC6H texture, whose section type is
+ * textureFormat (HapGetFrameTextureFormat reports it).  Geometry as for the RGBA16F decoders: width and height multiples of
+ * 4, 8 * width <= rowBytes <= HAPB200_MAX_ROW_BYTES, at most HAPB200_MAX_BLOCKS blocks; the batch entry points take device
+ * pointers, with rows, pictures, strides, out and blocks 16-byte aligned, and any number of frames.  compressor and
+ * chunkCount as for HapB200EncodeRGBA.  The output of a frame needs
+ *     HapMaxEncodedLength(1, {(width/4)*(height/4)*16}, {textureFormat}, {chunkCount})
+ * bytes (outputBufferBytes, outStride); less is refused with HapResult_Buffer_Too_Small.
+ * Input rules, applied to R, G and B before the search:
+ *   UF16: negative values, -0 and NaN encode as 0; +Inf as 65504 (0x7BFF).
+ *   SF16: NaN encodes as 0; +-Inf as +-65504; -0 as +0.
+ * After them, a block whose 16 texels hold one colour decodes bit-exactly to that colour (mode 14, a 16-bit base with zero
+ * deltas, represents every finite half of either signedness).  Each block is chosen by its exact error after decoding:
+ * the squared difference of decoded and source halves taken as sign-magnitude integers, summed over R, G and B. */
+
+/* one RGBA16F picture (host or device pointers) -> one Hap HDR frame */
+unsigned int HapB200EncodeRGBAHalf(const void *rgbaHalf, unsigned int width, unsigned int height, unsigned long rowBytes,
+                                   unsigned int textureFormat, unsigned int compressor, unsigned int chunkCount,
+                                   void *outputBuffer, unsigned long outputBufferBytes, unsigned long *outputBufferBytesUsed);
+/* frames x RGBA16F (device) -> frames x Hap HDR frame at out + f*outStride, encoded length in used[f] (device) */
+unsigned int HapB200EncodeRGBAHalfBatch(const void *rgbaHalf, unsigned int frames, unsigned long frameStride,
+                                        unsigned int width, unsigned int height, unsigned long rowBytes,
+                                        unsigned int textureFormat, unsigned int compressor, unsigned int chunkCount,
+                                        void *out, unsigned long outStride, unsigned long long *used, void *stream);
+/* frames x RGBA16F (device) -> bare BC6H textures at blocks + f*blocksStride */
+unsigned int HapB200BlockEncodeHalfBatch(const void *rgbaHalf, unsigned int frames, unsigned long frameStride,
+                                         unsigned int width, unsigned int height, unsigned long rowBytes,
+                                         unsigned int textureFormat, void *blocks, unsigned long blocksStride, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -108,6 +108,10 @@ HAP_HD uint32_t bc7_expand(uint32_t v, uint32_t n) { return (v << (8 - n)) | (v 
 // i * 4095 / (2^b - 1) = i * {1365, 585, 273}.
 HAP_HD uint32_t bc7_weight(uint32_t i, uint32_t b) { return (i * (b == 2 ? 1365u : b == 3 ? 585u : 273u) + 32u) >> 6; }
 
+// One 8-bit channel between endpoint values e0 and e1 at weight w (of 64), as the format interpolates: the expression
+// bc7_decode_block evaluates for G and A (and for R and B two at a time in 16-bit lanes), for the encoder's error
+HAP_HD uint32_t bc7_interp(uint32_t e0, uint32_t e1, uint32_t w) { return ((64 - w) * e0 + w * e1 + 32u) >> 6; }
+
 // One block -> its 16 texels, packed RGBA (texel t = row t/4, column t%4)
 HAP_HD void bc7_decode_block(uint32_t w0, uint32_t w1, uint32_t w2, uint32_t w3, uint32_t out[16])
 {

@@ -8,10 +8,12 @@
 // the order hap.c:450 slices into chunks.
 #pragma once
 #include "bc_block.cuh"
+#include "bc7_encode.cuh"
 
 namespace hapb200 {
 
-// kBcBc7 (BPTC RGBA UNORM, Hap R) is decoded only (bc7_decode.cuh): there is no BC7 block compressor
+// kBcBc7: BPTC RGBA UNORM (Hap R), block math in bc7_encode.cuh (encode) and bc7_decode.cuh (decode).  The codec-taking RGBA
+// encode entry points refuse it; the BC7 entry points ask for it by name.
 enum BcKind : int { kBcDxt1 = 0, kBcDxt5 = 1, kBcYCoCg = 2, kBcRgtc1 = 3, kBcYCoCgPlusAlpha = 4, kBcBc7 = 5 };
 
 constexpr int kBcThreads = 128;
@@ -51,9 +53,10 @@ HAP_HD uint32_t bc_ctas(uint32_t blocks_x, uint32_t blocks_y) { return (uint32_t
 // The frame is blockIdx.y, and gridDim.y is at most 65535: batches of more frames are launched in slices of this many.
 constexpr uint32_t kBcFramesPerLaunch = 65535;
 
-// grid = (bc_ctas, frames).  REFINE: the chroma endpoint refinement of the YCoCg kinds (bc_block.cuh).
+// grid = (bc_ctas, frames).  REFINE: the chroma endpoint refinement of the YCoCg kinds (bc_block.cuh).  kBcBc7 asks for one
+// resident CTA (a cap of 255 registers): its exact-error search holds more state than any register cap would keep.
 template <int KIND, bool REFINE = false>
-__global__ void __launch_bounds__(kBcThreads, (KIND == kBcYCoCg && !REFINE) ? 7 : (KIND == kBcDxt1 || KIND == kBcDxt5) ? 5 : HAPB200_BC_MIN_BLOCKS) bc_encode_kernel(const uint8_t *__restrict__ rgba, BcGeom G,
+__global__ void __launch_bounds__(kBcThreads, (KIND == kBcYCoCg && !REFINE) ? 7 : (KIND == kBcDxt1 || KIND == kBcDxt5) ? 5 : KIND == kBcBc7 ? 1 : HAPB200_BC_MIN_BLOCKS) bc_encode_kernel(const uint8_t *__restrict__ rgba, BcGeom G,
                                                                 uint8_t *__restrict__ out)
 {
     const uint32_t nblocks = G.blocks_x * G.blocks_y;
@@ -79,6 +82,10 @@ __global__ void __launch_bounds__(kBcThreads, (KIND == kBcYCoCg && !REFINE) ? 7 
         Block8 a, c;
         encode_dxt5(px, a, c);
         reinterpret_cast<uint4 *>(o)[bi] = make_uint4(a.lo, a.hi, c.lo, c.hi);
+    } else if (KIND == kBcBc7) {
+        uint32_t w[4];
+        bc7_encode_block(px, w);
+        reinterpret_cast<uint4 *>(o)[bi] = make_uint4(w[0], w[1], w[2], w[3]);
     } else {
         Block8 a, c;
         encode_ycocg_dxt5<REFINE>(px, a, c);

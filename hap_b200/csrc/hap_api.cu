@@ -365,7 +365,8 @@ uint32_t launch_block_encode(const uint8_t *rgba, uint32_t frames, uint64_t fram
     case kBcYCoCg: launch_bc_encode<kBcYCoCg>(frames, st, rgba, g, blocks, refine); break;
     case kBcRgtc1: launch_bc_encode<kBcRgtc1>(frames, st, rgba, g, blocks, refine); break;
     case kBcYCoCgPlusAlpha: launch_bc_encode<kBcYCoCgPlusAlpha>(frames, st, rgba, g, blocks, refine); break;
-    default: return HapResult_Bad_Arguments;   // kBcBc7: no block compressor (the entry points refuse it first)
+    case kBcBc7: launch_bc_encode<kBcBc7>(frames, st, rgba, g, blocks, refine); break;
+    default: return HapResult_Bad_Arguments;
     }
     return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
 }
@@ -1092,21 +1093,91 @@ unsigned int HapDecode(const void *inputBuffer, unsigned long inputBufferBytes, 
 
 // ---- extensions ----------------------------------------------------------------------------------
 
+static unsigned long texture_bytes(unsigned width, unsigned height, const CodecInfo &ci, unsigned index)
+{
+    if (index >= ci.textures || width % 4 || height % 4) return 0;
+    return (unsigned long)(width / 4) * (height / 4) * ci.block_bytes[index];
+}
+
+static unsigned long max_encoded_length_rgba(unsigned width, unsigned height, const CodecInfo &ci, unsigned chunkCount)
+{
+    unsigned long lens[2] = {texture_bytes(width, height, ci, 0), texture_bytes(width, height, ci, 1)};
+    unsigned fmts[2] = {ci.fmt[0], ci.fmt[1]}, chunks[2] = {chunkCount, chunkCount};
+    if (lens[0] == 0) return 0;
+    return HapMaxEncodedLength(ci.textures, lens, fmts, chunks);
+}
+
 unsigned long HapB200TextureBytes(unsigned int width, unsigned int height, unsigned int codec, unsigned int index)
 {
     CodecInfo ci;
-    if (!codec_info(codec, ci) || index >= ci.textures || width % 4 || height % 4) return 0;
-    return (unsigned long)(width / 4) * (height / 4) * ci.block_bytes[index];
+    if (!codec_info(codec, ci)) return 0;
+    return texture_bytes(width, height, ci, index);
 }
 
 unsigned long HapB200MaxEncodedLengthRGBA(unsigned int width, unsigned int height, unsigned int codec, unsigned int chunkCount)
 {
     CodecInfo ci;
     if (!codec_info(codec, ci)) return 0;
-    unsigned long lens[2] = {HapB200TextureBytes(width, height, codec, 0), HapB200TextureBytes(width, height, codec, 1)};
-    unsigned fmts[2] = {ci.fmt[0], ci.fmt[1]}, chunks[2] = {chunkCount, chunkCount};
-    if (lens[0] == 0) return 0;
-    return HapMaxEncodedLength(ci.textures, lens, fmts, chunks);
+    return max_encoded_length_rgba(width, height, ci, chunkCount);
+}
+
+// The RGBA8 encoders of every codec with a block compressor, behind the codec-taking entry points (which refuse Hap7) and the
+// BC7 ones (which ask for it by name)
+static unsigned block_encode_rgba_batch(const CodecInfo &ci, const void *rgba, unsigned frames, unsigned long frameStride, unsigned width,
+                                        unsigned height, unsigned long rowBytes, void *blocks, unsigned long blocksStride, void *stream)
+{
+    if (!blocks || frames == 0 || !rgba_geometry_ok(rgba, width, height, rowBytes, frameStride, true) || ((uintptr_t)blocks | blocksStride) % 16)
+        return HapResult_Bad_Arguments;
+    HAP_ENTER(rgba, blocks);
+    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
+        return launch_block_encode((const uint8_t *)rgba, frames, frameStride, width, height, rowBytes, ci, (uint8_t *)blocks, blocksStride,
+                                   texture_bytes(width, height, ci, 0), st);
+    });
+}
+
+static unsigned encode_rgba_batch(const CodecInfo &ci, const void *rgba, unsigned frames, unsigned long frameStride, unsigned width,
+                                  unsigned height, unsigned long rowBytes, unsigned compressor, unsigned chunkCount, void *out,
+                                  unsigned long outStride, unsigned long long *used, void *stream)
+{
+    if (!out || !used || frames == 0 || chunkCount == 0 || !rgba_geometry_ok(rgba, width, height, rowBytes, frameStride, true) ||
+        (compressor != HapCompressorNone && compressor != HapCompressorSnappy))
+        return HapResult_Bad_Arguments;
+    if (outStride < max_encoded_length_rgba(width, height, ci, chunkCount)) return HapResult_Buffer_Too_Small;
+    HAP_ENTER(rgba, out);
+    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
+        const uint64_t t[2] = {texture_bytes(width, height, ci, 0), texture_bytes(width, height, ci, 1)};
+        return encode_frames_from_blocks(frames, ci.textures, t, ci.fmt, compressor, chunkCount, (uint8_t *)out, outStride, used, st,
+                                         [&](uint8_t *tex, uint64_t stride) {
+                                             return launch_block_encode((const uint8_t *)rgba, frames, frameStride, width, height, rowBytes, ci,
+                                                                        tex, stride, align16(t[0]), st);
+                                         });
+    });
+}
+
+static unsigned encode_rgba(const CodecInfo &ci, const void *rgba, unsigned width, unsigned height, unsigned long rowBytes, unsigned compressor,
+                            unsigned chunkCount, void *outputBuffer, unsigned long outputBufferBytes, unsigned long *outputBufferBytesUsed)
+{
+    if (!outputBuffer || !outputBufferBytesUsed || chunkCount == 0 || !rgba_geometry_ok(rgba, width, height, rowBytes, 0, false) ||
+        (compressor != HapCompressorNone && compressor != HapCompressorSnappy))
+        return HapResult_Bad_Arguments;
+    const unsigned long cap = max_encoded_length_rgba(width, height, ci, chunkCount);
+    if (outputBufferBytes < cap) return HapResult_Buffer_Too_Small;
+    HAP_ENTER(rgba, outputBuffer);
+    CallStream call(!is_device(rgba) && !is_device(outputBuffer));
+    cudaStream_t st = call.st;
+    DevBuf img(st), frame(st), used(st);
+    const uint64_t tight = 4ull * width;
+    if (!img.alloc(tight * height) || !frame.alloc(cap) || !used.alloc(32)) { cudaGetLastError(); return HapResult_Internal_Error; }
+    if (cudaMemcpy2DAsync(img.p, tight, rgba, rowBytes, tight, height, cudaMemcpyDefault, st) != cudaSuccess) { cudaGetLastError(); return HapResult_Internal_Error; }
+    uint32_t r = encode_rgba_batch(ci, img.p, 1, align16(tight * height), width, height, tight, compressor, chunkCount, frame.p, cap,
+                                   used.as<unsigned long long>(), st);
+    if (r != HapResult_No_Error) return r;
+    unsigned long long total = 0;
+    if (cudaMemcpyAsync(&total, used.p, sizeof total, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess ||
+        total > outputBufferBytes || cudaMemcpyAsync(outputBuffer, frame.p, total, cudaMemcpyDefault, st) != cudaSuccess ||
+        cudaStreamSynchronize(st) != cudaSuccess) { cudaGetLastError(); return HapResult_Internal_Error; }
+    *outputBufferBytesUsed = (unsigned long)total;
+    return HapResult_No_Error;
 }
 
 unsigned int HapB200BlockEncodeBatch(const void *rgba, unsigned int frames, unsigned long frameStride, unsigned int width,
@@ -1114,14 +1185,8 @@ unsigned int HapB200BlockEncodeBatch(const void *rgba, unsigned int frames, unsi
                                      unsigned long blocksStride, void *stream)
 {
     CodecInfo ci;
-    if (!blocks || frames == 0 || !codec_info(codec, ci) || !codec_encodes(ci) ||
-        !rgba_geometry_ok(rgba, width, height, rowBytes, frameStride, true) || ((uintptr_t)blocks | blocksStride) % 16)
-        return HapResult_Bad_Arguments;
-    HAP_ENTER(rgba, blocks);
-    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
-        return launch_block_encode((const uint8_t *)rgba, frames, frameStride, width, height, rowBytes, ci, (uint8_t *)blocks, blocksStride,
-                                   HapB200TextureBytes(width, height, codec, 0), st);
-    });
+    if (!codec_info(codec, ci) || !codec_encodes(ci)) return HapResult_Bad_Arguments;
+    return block_encode_rgba_batch(ci, rgba, frames, frameStride, width, height, rowBytes, blocks, blocksStride, stream);
 }
 
 unsigned int HapB200BlockDecodeBatch(const void *blocks, unsigned int frames, unsigned long blocksStride, unsigned int width,
@@ -1174,19 +1239,8 @@ unsigned int HapB200EncodeRGBABatch(const void *rgba, unsigned int frames, unsig
                                     void *stream)
 {
     CodecInfo ci;
-    if (!out || !used || frames == 0 || chunkCount == 0 || !codec_info(codec, ci) || !codec_encodes(ci) ||
-        !rgba_geometry_ok(rgba, width, height, rowBytes, frameStride, true) || (compressor != HapCompressorNone && compressor != HapCompressorSnappy))
-        return HapResult_Bad_Arguments;
-    if (outStride < HapB200MaxEncodedLengthRGBA(width, height, codec, chunkCount)) return HapResult_Buffer_Too_Small;
-    HAP_ENTER(rgba, out);
-    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
-        const uint64_t t[2] = {HapB200TextureBytes(width, height, codec, 0), HapB200TextureBytes(width, height, codec, 1)};
-        return encode_frames_from_blocks(frames, ci.textures, t, ci.fmt, compressor, chunkCount, (uint8_t *)out, outStride, used, st,
-                                         [&](uint8_t *tex, uint64_t stride) {
-                                             return launch_block_encode((const uint8_t *)rgba, frames, frameStride, width, height, rowBytes, ci,
-                                                                        tex, stride, align16(t[0]), st);
-                                         });
-    });
+    if (!codec_info(codec, ci) || !codec_encodes(ci)) return HapResult_Bad_Arguments;
+    return encode_rgba_batch(ci, rgba, frames, frameStride, width, height, rowBytes, compressor, chunkCount, out, outStride, used, stream);
 }
 
 unsigned int HapB200EncodeRGBA(const void *rgba, unsigned int width, unsigned int height, unsigned long rowBytes,
@@ -1194,27 +1248,38 @@ unsigned int HapB200EncodeRGBA(const void *rgba, unsigned int width, unsigned in
                                unsigned long outputBufferBytes, unsigned long *outputBufferBytesUsed)
 {
     CodecInfo ci;
-    if (!outputBuffer || !outputBufferBytesUsed || chunkCount == 0 || !codec_info(codec, ci) || !codec_encodes(ci) ||
-        !rgba_geometry_ok(rgba, width, height, rowBytes, 0, false) || (compressor != HapCompressorNone && compressor != HapCompressorSnappy))
-        return HapResult_Bad_Arguments;
-    const unsigned long cap = HapB200MaxEncodedLengthRGBA(width, height, codec, chunkCount);
-    if (outputBufferBytes < cap) return HapResult_Buffer_Too_Small;
-    HAP_ENTER(rgba, outputBuffer);
-    CallStream call(!is_device(rgba) && !is_device(outputBuffer));
-    cudaStream_t st = call.st;
-    DevBuf img(st), frame(st), used(st);
-    const uint64_t tight = 4ull * width;
-    if (!img.alloc(tight * height) || !frame.alloc(cap) || !used.alloc(32)) { cudaGetLastError(); return HapResult_Internal_Error; }
-    if (cudaMemcpy2DAsync(img.p, tight, rgba, rowBytes, tight, height, cudaMemcpyDefault, st) != cudaSuccess) { cudaGetLastError(); return HapResult_Internal_Error; }
-    uint32_t r = HapB200EncodeRGBABatch(img.p, 1, align16(tight * height), width, height, tight, codec, compressor, chunkCount,
-                                        frame.p, cap, used.as<unsigned long long>(), st);
-    if (r != HapResult_No_Error) return r;
-    unsigned long long total = 0;
-    if (cudaMemcpyAsync(&total, used.p, sizeof total, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess ||
-        total > outputBufferBytes || cudaMemcpyAsync(outputBuffer, frame.p, total, cudaMemcpyDefault, st) != cudaSuccess ||
-        cudaStreamSynchronize(st) != cudaSuccess) { cudaGetLastError(); return HapResult_Internal_Error; }
-    *outputBufferBytesUsed = (unsigned long)total;
-    return HapResult_No_Error;
+    if (!codec_info(codec, ci) || !codec_encodes(ci)) return HapResult_Bad_Arguments;
+    return encode_rgba(ci, rgba, width, height, rowBytes, compressor, chunkCount, outputBuffer, outputBufferBytes, outputBufferBytesUsed);
+}
+
+// ---- Hap R encoding: RGBA8 -> BC7 (bc7_encode.cuh), the RGBA8 encoders' plumbing with the Hap7 codec -------------------
+
+static CodecInfo bc7_codec()
+{
+    CodecInfo ci;
+    codec_info(HapB200Codec_Hap7, ci);
+    return ci;
+}
+
+unsigned int HapB200EncodeRGBABC7(const void *rgba, unsigned int width, unsigned int height, unsigned long rowBytes,
+                                  unsigned int compressor, unsigned int chunkCount, void *outputBuffer,
+                                  unsigned long outputBufferBytes, unsigned long *outputBufferBytesUsed)
+{
+    return encode_rgba(bc7_codec(), rgba, width, height, rowBytes, compressor, chunkCount, outputBuffer, outputBufferBytes, outputBufferBytesUsed);
+}
+
+unsigned int HapB200EncodeRGBABC7Batch(const void *rgba, unsigned int frames, unsigned long frameStride, unsigned int width,
+                                       unsigned int height, unsigned long rowBytes, unsigned int compressor, unsigned int chunkCount,
+                                       void *out, unsigned long outStride, unsigned long long *used, void *stream)
+{
+    return encode_rgba_batch(bc7_codec(), rgba, frames, frameStride, width, height, rowBytes, compressor, chunkCount, out, outStride, used,
+                             stream);
+}
+
+unsigned int HapB200BlockEncodeBC7Batch(const void *rgba, unsigned int frames, unsigned long frameStride, unsigned int width,
+                                        unsigned int height, unsigned long rowBytes, void *blocks, unsigned long blocksStride, void *stream)
+{
+    return block_encode_rgba_batch(bc7_codec(), rgba, frames, frameStride, width, height, rowBytes, blocks, blocksStride, stream);
 }
 
 unsigned int HapB200DecodeBatch(const void *in, unsigned int frames, unsigned long inStride, const unsigned long long *inBytes,

@@ -10,7 +10,8 @@ from .abi import HapABI
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 HapB200Codec_Hap1, HapB200Codec_Hap5, HapB200Codec_HapY, HapB200Codec_HapM, HapB200Codec_HapA, HapB200Codec_Hap7 = range(6)
-# HapB200Codec_Hap7 ("Hap R", BC7) decodes only: the RGBA encode entry points refuse it with HapResult_Bad_Arguments
+# HapB200Codec_Hap7 ("Hap R", BC7): the codec-taking RGBA encode entry points refuse it with HapResult_Bad_Arguments; the
+# BC7 encoders (encode_rgba_bc7, encode_rgba_bc7_batch, block_encode_bc7_batch) ask for it by name
 
 
 def library_path() -> str:
@@ -68,6 +69,12 @@ class HapB200(HapABI):
         L.HapB200EncodeRGBAHalfBatch.restype = u
         L.HapB200EncodeRGBAHalfBatch.argtypes = [vp, u, ul, u, u, ul, u, u, u, vp, ul, vp, vp]
         L.HapB200BlockEncodeHalfBatch.restype = u
+        L.HapB200EncodeRGBABC7.restype = u
+        L.HapB200EncodeRGBABC7.argtypes = [vp, u, u, ul, u, u, vp, ul, C.POINTER(ul)]
+        L.HapB200EncodeRGBABC7Batch.restype = u
+        L.HapB200EncodeRGBABC7Batch.argtypes = [vp, u, ul, u, u, ul, u, u, vp, ul, vp, vp]
+        L.HapB200BlockEncodeBC7Batch.restype = u
+        L.HapB200BlockEncodeBC7Batch.argtypes = [vp, u, ul, u, u, ul, vp, ul, vp]
         L.HapB200BlockEncodeHalfBatch.argtypes = [vp, u, ul, u, u, ul, u, vp, ul, vp]
         for name, args in (("RingCreate", [C.c_int, ul, C.POINTER(vp), vp]), ("RingDestroy", [C.c_int, vp]),
                            ("RingOpen", [C.c_int, vp, C.POINTER(vp)]), ("RingClose", [C.c_int, vp]),
@@ -238,6 +245,30 @@ class HapB200(HapABI):
         return int(self.lib.HapB200BlockEncodeHalfBatch(rgba, frames, frame_stride, w, h, row_bytes or 8 * w, texture_format,
                                                         blocks, blocks_stride, stream))
 
+    # -- RGBA8 -> Hap R (BC7): frames need max_encoded_length_rgba(w, h, HapB200Codec_Hap7, chunks) --------------------------
+    def encode_rgba_bc7(self, rgba, w, h, compressor=1, chunks=1, row_bytes=None, out=None, out_capacity=None):
+        """rgba: buffer object or (addr, nbytes), 4 bytes per pixel.  Returns (result, frame bytes | used)."""
+        from .abi import _as_ptr
+        addr, _ = _as_ptr(rgba)
+        cap = self.max_encoded_length_rgba(w, h, HapB200Codec_Hap7, chunks) if out_capacity is None else out_capacity
+        own = out is None
+        if own:
+            out = bytearray(max(cap, 1))
+        oaddr, _ = _as_ptr(out)
+        used = C.c_ulong(0)
+        r = self.lib.HapB200EncodeRGBABC7(addr, w, h, row_bytes or 4 * w, compressor, chunks, oaddr, cap, C.byref(used))
+        if r != 0:
+            return int(r), None
+        return 0, (bytes(memoryview(out)[: used.value]) if own else used.value)
+
+    def encode_rgba_bc7_batch(self, rgba, frames, frame_stride, w, h, compressor, chunks, out, out_stride, used, row_bytes=None,
+                              stream=None):
+        return int(self.lib.HapB200EncodeRGBABC7Batch(rgba, frames, frame_stride, w, h, row_bytes or 4 * w, compressor, chunks, out,
+                                                      out_stride, used, stream))
+
+    def block_encode_bc7_batch(self, rgba, frames, frame_stride, w, h, blocks, blocks_stride, row_bytes=None, stream=None):
+        return int(self.lib.HapB200BlockEncodeBC7Batch(rgba, frames, frame_stride, w, h, row_bytes or 4 * w, blocks, blocks_stride,
+                                                       stream))
 
     # -- delivery rings (include/hap_b200.h): frames written straight into another GPU's memory -----------------
     RING_HANDLE_BYTES = 64

@@ -26,9 +26,10 @@ enum HapB200Codec {
     HapB200Codec_HapA = 4, /* alpha RGTC1                      "Hap Alpha-Only" */
     HapB200Codec_Hap7 = 5  /* RGBA BPTC (BC7) UNORM            "Hap R"          */
 };
-/* Hap R (Hap7) is decode-only: the library has no BC7 block compressor.  HapB200EncodeRGBA, HapB200EncodeRGBABatch and
- * HapB200BlockEncodeBatch refuse it with HapResult_Bad_Arguments; HapEncode and HapB200EncodeBatch wrap BC7 textures that
- * were compressed elsewhere.  The RGBA decoders turn BC7 blocks into RGBA8 exactly as the BPTC specification defines them,
+/* Hap R (Hap7): the codec-taking encoders HapB200EncodeRGBA, HapB200EncodeRGBABatch and HapB200BlockEncodeBatch refuse it
+ * with HapResult_Bad_Arguments (a BC7 search costs far more per block than the DXT encoders, so a caller asks for it by
+ * name): HapB200EncodeRGBABC7, HapB200EncodeRGBABC7Batch and HapB200BlockEncodeBC7Batch encode it.  HapEncode and
+ * HapB200EncodeBatch wrap BC7 textures that were compressed elsewhere.  The RGBA decoders turn BC7 blocks into RGBA8 exactly as the BPTC specification defines them,
  * reserved blocks (first byte 0) included: those decode to (0, 0, 0, 0) in all 16 texels. */
 
 const char *HapB200Version(void);
@@ -153,7 +154,7 @@ unsigned int HapB200DecodeRGBABatch(const void *in, unsigned int frames, unsigne
                                     void *stream);
 
 /* Block codecs alone (K1-K4 / K8), batched: kind = HapB200Codec; HapM writes/reads the YCoCg plane at
- * blocks and the RGTC1 plane at blocks + HapB200TextureBytes(.., 0).  Hap7 (BC7) decodes only.  BC6H blocks: see
+ * blocks and the RGTC1 plane at blocks + HapB200TextureBytes(.., 0).  Hap7 (BC7) decodes only here (encode: HapB200BlockEncodeBC7Batch).  BC6H blocks: see
  * HapB200BlockDecodeHalfBatch. */
 unsigned int HapB200BlockEncodeBatch(const void *rgba, unsigned int frames, unsigned long frameStride,
                                      unsigned int width, unsigned int height, unsigned long rowBytes,
@@ -220,6 +221,35 @@ unsigned int HapB200EncodeRGBAHalfBatch(const void *rgbaHalf, unsigned int frame
 unsigned int HapB200BlockEncodeHalfBatch(const void *rgbaHalf, unsigned int frames, unsigned long frameStride,
                                          unsigned int width, unsigned int height, unsigned long rowBytes,
                                          unsigned int textureFormat, void *blocks, unsigned long blocksStride, void *stream);
+
+/* ---- Hap R (BC7, "Hap7") <- RGBA8 ----------------------------------------------------------------------------------------
+ * The encoders take RGBA8 pictures and write BPTC (BC7) RGBA UNORM blocks.  Geometry, alignment, compressor and chunkCount as
+ * for HapB200EncodeRGBA / HapB200EncodeRGBABatch / HapB200BlockEncodeBatch.  A frame holds one texture of format
+ * HapTextureFormat_RGBA_BPTC_UNORM and needs HapB200MaxEncodedLengthRGBA(width, height, HapB200Codec_Hap7, chunkCount)
+ * bytes (outputBufferBytes, outStride); less is refused with HapResult_Buffer_Too_Small.  Arguments are checked before
+ * anything touches the GPU.
+ * Each block is chosen by its exact error after decoding: the sum over R, G, B and A of the squared differences of decoded
+ * and source 8-bit values, unweighted.  Rules:
+ *   - a block whose 16 texels hold one RGBA colour decodes bit-exactly to that colour (mode 5, rotation 0, colour index 1
+ *     between two 7-bit endpoints per channel, both alpha endpoints at A);
+ *   - a block whose texels all have A = 255 decodes with A = 255 in all 16 texels (modes 0-3 always do; modes 4-7 keep the
+ *     channel that decodes to A at its top code, in modes 6 and 7 with p-bits 1);
+ *   - no reserved block (first byte 0) is ever written.
+ * A BC7 search costs orders of magnitude more per block than the DXT encoders (DESIGN.md section 6). */
+
+/* one RGBA8 picture (host or device pointers) -> one Hap R frame */
+unsigned int HapB200EncodeRGBABC7(const void *rgba, unsigned int width, unsigned int height, unsigned long rowBytes,
+                                  unsigned int compressor, unsigned int chunkCount,
+                                  void *outputBuffer, unsigned long outputBufferBytes, unsigned long *outputBufferBytesUsed);
+/* frames x RGBA8 (device) -> frames x Hap R frame at out + f*outStride, encoded length in used[f] (device) */
+unsigned int HapB200EncodeRGBABC7Batch(const void *rgba, unsigned int frames, unsigned long frameStride,
+                                       unsigned int width, unsigned int height, unsigned long rowBytes,
+                                       unsigned int compressor, unsigned int chunkCount,
+                                       void *out, unsigned long outStride, unsigned long long *used, void *stream);
+/* frames x RGBA8 (device) -> bare BC7 textures at blocks + f*blocksStride */
+unsigned int HapB200BlockEncodeBC7Batch(const void *rgba, unsigned int frames, unsigned long frameStride,
+                                        unsigned int width, unsigned int height, unsigned long rowBytes,
+                                        void *blocks, unsigned long blocksStride, void *stream);
 
 #ifdef __cplusplus
 }

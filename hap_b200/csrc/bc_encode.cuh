@@ -1,4 +1,4 @@
-// hap_b200/csrc/bc_encode.cuh -- K1-K4 kernels: RGBA8 frames -> DXT1 / DXT5 / scaled-YCoCg-DXT5 / RGTC1 blocks.
+// hap_b200/csrc/bc_encode.cuh -- K1-K4 kernels: RGBA8 (or NV12 / P010) frames -> DXT1 / DXT5 / scaled-YCoCg-DXT5 / RGTC1 blocks.
 //
 // One thread per 4x4 block (see bc_block.cuh for why).  Memory shape: thread t of a warp owns block
 // column bx0+t, so for each of the four pixel rows the warp reads 32 x 16 B = 512 contiguous bytes
@@ -9,6 +9,7 @@
 #pragma once
 #include "bc_block.cuh"
 #include "bc7_encode.cuh"
+#include "yuv_source.cuh"
 
 namespace hapb200 {
 
@@ -55,21 +56,29 @@ constexpr uint32_t kBcFramesPerLaunch = 65535;
 
 // grid = (bc_ctas, frames).  REFINE: the chroma endpoint refinement of the YCoCg kinds (bc_block.cuh).  kBcBc7 asks for one
 // resident CTA (a cap of 255 registers): its exact-error search holds more state than any register cap would keep.
-template <int KIND, bool REFINE = false>
+// SRC (BcSource): kSrcRgba8 reads `rgba` as RGBA8 rows; kSrcNv12 / kSrcP010 read it as the luma plane and Y.chroma as the
+// chroma plane (yuv_source.cuh), both frame_bytes apart per frame, and convert before the fit.  Y comes last so that the
+// parameters of the RGBA8 instantiations keep their offsets.
+template <int KIND, bool REFINE = false, int SRC = kSrcRgba8>
 __global__ void __launch_bounds__(kBcThreads, (KIND == kBcYCoCg && !REFINE) ? 7 : (KIND == kBcDxt1 || KIND == kBcDxt5) ? 5 : KIND == kBcBc7 ? 1 : HAPB200_BC_MIN_BLOCKS) bc_encode_kernel(const uint8_t *__restrict__ rgba, BcGeom G,
-                                                                uint8_t *__restrict__ out)
+                                                                uint8_t *__restrict__ out, YuvSrc Y = YuvSrc())
 {
     const uint32_t nblocks = G.blocks_x * G.blocks_y;
     const uint32_t bi = blockIdx.x * kBcThreads + threadIdx.x;
     if (bi >= nblocks) return;
     uint32_t by = __umulhi(bi, G.inv_blocks_x), bx = bi - by * G.blocks_x;  // the estimate is exact or one short
     if (bx >= G.blocks_x) { by++; bx -= G.blocks_x; }
-    const uint8_t *src = rgba + (uint64_t)blockIdx.y * G.frame_bytes + (uint64_t)(4 * by) * G.row_bytes + 16u * bx;
     uint32_t px[16];
+    if (SRC == kSrcRgba8) {
+        const uint8_t *src = rgba + (uint64_t)blockIdx.y * G.frame_bytes + (uint64_t)(4 * by) * G.row_bytes + 16u * bx;
 #pragma unroll
-    for (int row = 0; row < 4; row++) {
-        uint4 v = *reinterpret_cast<const uint4 *>(src + (uint64_t)row * G.row_bytes);
-        px[4 * row + 0] = v.x; px[4 * row + 1] = v.y; px[4 * row + 2] = v.z; px[4 * row + 3] = v.w;
+        for (int row = 0; row < 4; row++) {
+            uint4 v = *reinterpret_cast<const uint4 *>(src + (uint64_t)row * G.row_bytes);
+            px[4 * row + 0] = v.x; px[4 * row + 1] = v.y; px[4 * row + 2] = v.z; px[4 * row + 3] = v.w;
+        }
+    } else {
+        const uint64_t f = (uint64_t)blockIdx.y * G.frame_bytes;
+        load_block_yuv<SRC>(rgba + f, Y.chroma + f, G.row_bytes, bx, by, G.blocks_x, G.blocks_y, Y, px);
     }
     uint8_t *o = out + (uint64_t)blockIdx.y * G.out_stride;
     if (KIND == kBcDxt1) {

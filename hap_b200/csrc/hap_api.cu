@@ -339,33 +339,51 @@ uint32_t launch_encode(const uint8_t *base, const FrameGeom &G, uint32_t frames,
     return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
 }
 
-// the scaled-YCoCg kinds have a chroma-refining variant (HAPB200_OPTION_CHROMA_REFINE).  One launch per kBcFramesPerLaunch frames.
-template <int KIND>
-void launch_bc_encode(uint32_t frames, cudaStream_t st, const uint8_t *rgba, const BcGeom &g, uint8_t *blocks, bool refine)
+// the scaled-YCoCg kinds have a chroma-refining variant (HAPB200_OPTION_CHROMA_REFINE)
+template <int KIND, int SRC>
+void launch_bc_encode_slice(const dim3 &grid, cudaStream_t st, const uint8_t *src, const BcGeom &g, uint8_t *dst, bool refine, const YuvSrc &yuv)
 {
     constexpr bool kRefines = KIND == kBcYCoCg || KIND == kBcYCoCgPlusAlpha;
+    if (kRefines && refine) HAP_KLAUNCH(kStBcEncode, (bc_encode_kernel<KIND, kRefines, SRC>), grid, dim3(kBcThreads), 0, st, src, g, dst, yuv);
+    else HAP_KLAUNCH(kStBcEncode, (bc_encode_kernel<KIND, false, SRC>), grid, dim3(kBcThreads), 0, st, src, g, dst, yuv);
+}
+
+// One launch per kBcFramesPerLaunch frames.  The kinds that encode colour (not RGTC1 alone, not BC7) also read NV12 / P010.
+template <int KIND>
+void launch_bc_encode(uint32_t frames, cudaStream_t st, const uint8_t *rgba, const BcGeom &g, uint8_t *blocks, bool refine, int src,
+                      const YuvSrc &yuv)
+{
+    constexpr bool kTakesYuv = KIND != kBcRgtc1 && KIND != kBcBc7;
     for (uint32_t f0 = 0; f0 < frames; f0 += kBcFramesPerLaunch) {
         const dim3 grid(bc_ctas(g.blocks_x, g.blocks_y), frames - f0 < kBcFramesPerLaunch ? frames - f0 : kBcFramesPerLaunch);
-        const uint8_t *src = rgba + f0 * g.frame_bytes;
+        const uint8_t *s = rgba + f0 * g.frame_bytes;
         uint8_t *dst = blocks + f0 * g.out_stride;
-        if (kRefines && refine) HAP_KLAUNCH(kStBcEncode, (bc_encode_kernel<KIND, kRefines>), grid, dim3(kBcThreads), 0, st, src, g, dst);
-        else HAP_KLAUNCH(kStBcEncode, bc_encode_kernel<KIND>, grid, dim3(kBcThreads), 0, st, src, g, dst);
+        YuvSrc y = yuv;
+        if (y.chroma) y.chroma += f0 * g.frame_bytes;
+        if constexpr (kTakesYuv) {
+            if (src == kSrcNv12) { launch_bc_encode_slice<KIND, kSrcNv12>(grid, st, s, g, dst, refine, y); continue; }
+            if (src == kSrcP010) { launch_bc_encode_slice<KIND, kSrcP010>(grid, st, s, g, dst, refine, y); continue; }
+        }
+        launch_bc_encode_slice<KIND, kSrcRgba8>(grid, st, s, g, dst, refine, y);
     }
 }
 
+// src (BcSource): kSrcRgba8 reads `rgba` as RGBA8 rows row_bytes apart; kSrcNv12 / kSrcP010 read it as the luma plane and
+// yuv.chroma as the chroma plane, both with pitch row_bytes.
 uint32_t launch_block_encode(const uint8_t *rgba, uint32_t frames, uint64_t frame_stride, uint32_t width, uint32_t height,
                              uint64_t row_bytes, const CodecInfo &ci, uint8_t *blocks, uint64_t blocks_stride,
-                             uint64_t second_offset, cudaStream_t st)
+                             uint64_t second_offset, cudaStream_t st, int src = kSrcRgba8, const YuvSrc &yuv = YuvSrc())
 {
     const BcGeom g = bc_encode_geom(width, height, (uint32_t)row_bytes, frame_stride, blocks_stride, second_offset);   // (rgba_geometry_ok: row_bytes < 2^32)
     const bool refine = g_chroma_refine.load() != 0;
+    if (src != kSrcRgba8 && (ci.bc_kind == kBcRgtc1 || ci.bc_kind == kBcBc7)) return HapResult_Bad_Arguments;
     switch (ci.bc_kind) {
-    case kBcDxt1: launch_bc_encode<kBcDxt1>(frames, st, rgba, g, blocks, refine); break;
-    case kBcDxt5: launch_bc_encode<kBcDxt5>(frames, st, rgba, g, blocks, refine); break;
-    case kBcYCoCg: launch_bc_encode<kBcYCoCg>(frames, st, rgba, g, blocks, refine); break;
-    case kBcRgtc1: launch_bc_encode<kBcRgtc1>(frames, st, rgba, g, blocks, refine); break;
-    case kBcYCoCgPlusAlpha: launch_bc_encode<kBcYCoCgPlusAlpha>(frames, st, rgba, g, blocks, refine); break;
-    case kBcBc7: launch_bc_encode<kBcBc7>(frames, st, rgba, g, blocks, refine); break;
+    case kBcDxt1: launch_bc_encode<kBcDxt1>(frames, st, rgba, g, blocks, refine, src, yuv); break;
+    case kBcDxt5: launch_bc_encode<kBcDxt5>(frames, st, rgba, g, blocks, refine, src, yuv); break;
+    case kBcYCoCg: launch_bc_encode<kBcYCoCg>(frames, st, rgba, g, blocks, refine, src, yuv); break;
+    case kBcRgtc1: launch_bc_encode<kBcRgtc1>(frames, st, rgba, g, blocks, refine, src, yuv); break;
+    case kBcYCoCgPlusAlpha: launch_bc_encode<kBcYCoCgPlusAlpha>(frames, st, rgba, g, blocks, refine, src, yuv); break;
+    case kBcBc7: launch_bc_encode<kBcBc7>(frames, st, rgba, g, blocks, refine, src, yuv); break;
     default: return HapResult_Bad_Arguments;
     }
     return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
@@ -1121,56 +1139,96 @@ unsigned long HapB200MaxEncodedLengthRGBA(unsigned int width, unsigned int heigh
     return max_encoded_length_rgba(width, height, ci, chunkCount);
 }
 
-// The RGBA8 encoders of every codec with a block compressor, behind the codec-taking entry points (which refuse Hap7) and the
-// BC7 ones (which ask for it by name)
-static unsigned block_encode_rgba_batch(const CodecInfo &ci, const void *rgba, unsigned frames, unsigned long frameStride, unsigned width,
-                                        unsigned height, unsigned long rowBytes, void *blocks, unsigned long blocksStride, void *stream)
+// The picture an encoder reads: an RGBA8 picture (kSrcRgba8), or the luma and chroma planes of an NV12 / P010 picture
+// (kSrcNv12 / kSrcP010, yuv_source.cuh).  Rows of both planes are `pitch` bytes apart.
+struct PictureSrc {
+    int kind;                 // BcSource
+    const void *pixels;       // the RGBA8 picture, or the luma plane
+    const void *chroma;       // the interleaved CbCr plane
+    unsigned color_space;     // HapB200YUVColorSpace
+    uint64_t sample_bytes() const { return kind == kSrcRgba8 ? 4 : kind == kSrcP010 ? 2 : 1; }   // per pixel of a luma / RGBA row
+    uint32_t planes() const { return kind == kSrcRgba8 ? 1 : 2; }
+    YuvSrc yuv() const { return kind == kSrcRgba8 ? YuvSrc() : yuv_src(kind - kSrcNv12, color_space, (const uint8_t *)chroma); }
+};
+PictureSrc rgba_picture(const void *rgba) { return {kSrcRgba8, rgba, nullptr, 0}; }
+
+// width x height NV12 (bpp 1) / P010 (bpp 2) planes with one pitch: the chroma plane's rows hold as many bytes as luma's.
+// aligned: the batch entry points' rules besides (16-byte aligned pitch, planes and frame stride).
+bool yuv_geometry_ok(const void *luma, const void *chroma, unsigned width, unsigned height, unsigned long pitch, unsigned long frameStride,
+                     bool aligned, unsigned long bpp)
 {
-    if (!blocks || frames == 0 || !rgba_geometry_ok(rgba, width, height, rowBytes, frameStride, true) || ((uintptr_t)blocks | blocksStride) % 16)
+    return chroma && rgba_geometry_ok(luma, width, height, pitch, frameStride, aligned, bpp) && (!aligned || (uintptr_t)chroma % 16 == 0);
+}
+
+bool picture_geometry_ok(const PictureSrc &p, unsigned width, unsigned height, unsigned long pitch, unsigned long frameStride, bool aligned)
+{
+    if (p.kind == kSrcRgba8) return rgba_geometry_ok(p.pixels, width, height, pitch, frameStride, aligned);
+    return yuv_geometry_ok(p.pixels, p.chroma, width, height, pitch, frameStride, aligned, p.sample_bytes());
+}
+
+// The picture encoders of every codec with a block compressor, behind the codec-taking RGBA8 entry points (which refuse
+// Hap7), the BC7 ones (which ask for it by name) and the YUV ones
+static unsigned block_encode_picture_batch(const CodecInfo &ci, const PictureSrc &p, unsigned frames, unsigned long frameStride,
+                                           unsigned width, unsigned height, unsigned long pitch, void *blocks, unsigned long blocksStride,
+                                           void *stream)
+{
+    if (!blocks || frames == 0 || !picture_geometry_ok(p, width, height, pitch, frameStride, true) || ((uintptr_t)blocks | blocksStride) % 16)
         return HapResult_Bad_Arguments;
-    HAP_ENTER(rgba, blocks);
+    HAP_ENTER(p.pixels, blocks);
     return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
-        return launch_block_encode((const uint8_t *)rgba, frames, frameStride, width, height, rowBytes, ci, (uint8_t *)blocks, blocksStride,
-                                   texture_bytes(width, height, ci, 0), st);
+        return launch_block_encode((const uint8_t *)p.pixels, frames, frameStride, width, height, pitch, ci, (uint8_t *)blocks, blocksStride,
+                                   texture_bytes(width, height, ci, 0), st, p.kind, p.yuv());
     });
 }
 
-static unsigned encode_rgba_batch(const CodecInfo &ci, const void *rgba, unsigned frames, unsigned long frameStride, unsigned width,
-                                  unsigned height, unsigned long rowBytes, unsigned compressor, unsigned chunkCount, void *out,
-                                  unsigned long outStride, unsigned long long *used, void *stream)
+static unsigned encode_picture_batch(const CodecInfo &ci, const PictureSrc &p, unsigned frames, unsigned long frameStride, unsigned width,
+                                     unsigned height, unsigned long pitch, unsigned compressor, unsigned chunkCount, void *out,
+                                     unsigned long outStride, unsigned long long *used, void *stream)
 {
-    if (!out || !used || frames == 0 || chunkCount == 0 || !rgba_geometry_ok(rgba, width, height, rowBytes, frameStride, true) ||
+    if (!out || !used || frames == 0 || chunkCount == 0 || !picture_geometry_ok(p, width, height, pitch, frameStride, true) ||
         (compressor != HapCompressorNone && compressor != HapCompressorSnappy))
         return HapResult_Bad_Arguments;
     if (outStride < max_encoded_length_rgba(width, height, ci, chunkCount)) return HapResult_Buffer_Too_Small;
-    HAP_ENTER(rgba, out);
+    HAP_ENTER(p.pixels, out);
     return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
         const uint64_t t[2] = {texture_bytes(width, height, ci, 0), texture_bytes(width, height, ci, 1)};
         return encode_frames_from_blocks(frames, ci.textures, t, ci.fmt, compressor, chunkCount, (uint8_t *)out, outStride, used, st,
                                          [&](uint8_t *tex, uint64_t stride) {
-                                             return launch_block_encode((const uint8_t *)rgba, frames, frameStride, width, height, rowBytes, ci,
-                                                                        tex, stride, align16(t[0]), st);
+                                             return launch_block_encode((const uint8_t *)p.pixels, frames, frameStride, width, height, pitch, ci,
+                                                                        tex, stride, align16(t[0]), st, p.kind, p.yuv());
                                          });
     });
 }
 
-static unsigned encode_rgba(const CodecInfo &ci, const void *rgba, unsigned width, unsigned height, unsigned long rowBytes, unsigned compressor,
-                            unsigned chunkCount, void *outputBuffer, unsigned long outputBufferBytes, unsigned long *outputBufferBytesUsed)
+// One picture in host or device memory: its planes are copied into tight device scratch (rows align16(row bytes) apart,
+// chroma after luma) and encoded as a batch of one.
+static unsigned encode_picture(const CodecInfo &ci, const PictureSrc &p, unsigned width, unsigned height, unsigned long pitch, unsigned compressor,
+                               unsigned chunkCount, void *outputBuffer, unsigned long outputBufferBytes, unsigned long *outputBufferBytesUsed)
 {
-    if (!outputBuffer || !outputBufferBytesUsed || chunkCount == 0 || !rgba_geometry_ok(rgba, width, height, rowBytes, 0, false) ||
+    if (!outputBuffer || !outputBufferBytesUsed || chunkCount == 0 || !picture_geometry_ok(p, width, height, pitch, 0, false) ||
         (compressor != HapCompressorNone && compressor != HapCompressorSnappy))
         return HapResult_Bad_Arguments;
     const unsigned long cap = max_encoded_length_rgba(width, height, ci, chunkCount);
     if (outputBufferBytes < cap) return HapResult_Buffer_Too_Small;
-    HAP_ENTER(rgba, outputBuffer);
-    CallStream call(!is_device(rgba) && !is_device(outputBuffer));
+    HAP_ENTER(p.pixels, outputBuffer);
+    CallStream call(!is_device(p.pixels) && !is_device(p.chroma) && !is_device(outputBuffer));
     cudaStream_t st = call.st;
     DevBuf img(st), frame(st), used(st);
-    const uint64_t tight = 4ull * width;
-    if (!img.alloc(tight * height) || !frame.alloc(cap) || !used.alloc(32)) { cudaGetLastError(); return HapResult_Internal_Error; }
-    if (cudaMemcpy2DAsync(img.p, tight, rgba, rowBytes, tight, height, cudaMemcpyDefault, st) != cudaSuccess) { cudaGetLastError(); return HapResult_Internal_Error; }
-    uint32_t r = encode_rgba_batch(ci, img.p, 1, align16(tight * height), width, height, tight, compressor, chunkCount, frame.p, cap,
-                                   used.as<unsigned long long>(), st);
+    const uint64_t row = p.sample_bytes() * width, tight = align16(row);   // (RGBA8: tight = row, width is a multiple of 4)
+    const uint64_t luma_bytes = tight * height, plane_bytes = luma_bytes + (p.planes() == 2 ? tight * (height / 2) : 0);
+    if (!img.alloc(plane_bytes) || !frame.alloc(cap) || !used.alloc(32)) { cudaGetLastError(); return HapResult_Internal_Error; }
+    PictureSrc dev = p;
+    dev.pixels = img.p;
+    if (cudaMemcpy2DAsync(img.p, tight, p.pixels, pitch, row, height, cudaMemcpyDefault, st) != cudaSuccess) { cudaGetLastError(); return HapResult_Internal_Error; }
+    if (p.planes() == 2) {
+        dev.chroma = img.as<uint8_t>() + luma_bytes;
+        if (cudaMemcpy2DAsync(img.as<uint8_t>() + luma_bytes, tight, p.chroma, pitch, row, height / 2, cudaMemcpyDefault, st) != cudaSuccess) {
+            cudaGetLastError();
+            return HapResult_Internal_Error;
+        }
+    }
+    uint32_t r = encode_picture_batch(ci, dev, 1, align16(plane_bytes), width, height, tight, compressor, chunkCount, frame.p, cap,
+                                      used.as<unsigned long long>(), st);
     if (r != HapResult_No_Error) return r;
     unsigned long long total = 0;
     if (cudaMemcpyAsync(&total, used.p, sizeof total, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess ||
@@ -1186,7 +1244,7 @@ unsigned int HapB200BlockEncodeBatch(const void *rgba, unsigned int frames, unsi
 {
     CodecInfo ci;
     if (!codec_info(codec, ci) || !codec_encodes(ci)) return HapResult_Bad_Arguments;
-    return block_encode_rgba_batch(ci, rgba, frames, frameStride, width, height, rowBytes, blocks, blocksStride, stream);
+    return block_encode_picture_batch(ci, rgba_picture(rgba), frames, frameStride, width, height, rowBytes, blocks, blocksStride, stream);
 }
 
 unsigned int HapB200BlockDecodeBatch(const void *blocks, unsigned int frames, unsigned long blocksStride, unsigned int width,
@@ -1240,7 +1298,7 @@ unsigned int HapB200EncodeRGBABatch(const void *rgba, unsigned int frames, unsig
 {
     CodecInfo ci;
     if (!codec_info(codec, ci) || !codec_encodes(ci)) return HapResult_Bad_Arguments;
-    return encode_rgba_batch(ci, rgba, frames, frameStride, width, height, rowBytes, compressor, chunkCount, out, outStride, used, stream);
+    return encode_picture_batch(ci, rgba_picture(rgba), frames, frameStride, width, height, rowBytes, compressor, chunkCount, out, outStride, used, stream);
 }
 
 unsigned int HapB200EncodeRGBA(const void *rgba, unsigned int width, unsigned int height, unsigned long rowBytes,
@@ -1249,7 +1307,7 @@ unsigned int HapB200EncodeRGBA(const void *rgba, unsigned int width, unsigned in
 {
     CodecInfo ci;
     if (!codec_info(codec, ci) || !codec_encodes(ci)) return HapResult_Bad_Arguments;
-    return encode_rgba(ci, rgba, width, height, rowBytes, compressor, chunkCount, outputBuffer, outputBufferBytes, outputBufferBytesUsed);
+    return encode_picture(ci, rgba_picture(rgba), width, height, rowBytes, compressor, chunkCount, outputBuffer, outputBufferBytes, outputBufferBytesUsed);
 }
 
 // ---- Hap R encoding: RGBA8 -> BC7 (bc7_encode.cuh), the RGBA8 encoders' plumbing with the Hap7 codec -------------------
@@ -1265,21 +1323,65 @@ unsigned int HapB200EncodeRGBABC7(const void *rgba, unsigned int width, unsigned
                                   unsigned int compressor, unsigned int chunkCount, void *outputBuffer,
                                   unsigned long outputBufferBytes, unsigned long *outputBufferBytesUsed)
 {
-    return encode_rgba(bc7_codec(), rgba, width, height, rowBytes, compressor, chunkCount, outputBuffer, outputBufferBytes, outputBufferBytesUsed);
+    return encode_picture(bc7_codec(), rgba_picture(rgba), width, height, rowBytes, compressor, chunkCount, outputBuffer, outputBufferBytes, outputBufferBytesUsed);
 }
 
 unsigned int HapB200EncodeRGBABC7Batch(const void *rgba, unsigned int frames, unsigned long frameStride, unsigned int width,
                                        unsigned int height, unsigned long rowBytes, unsigned int compressor, unsigned int chunkCount,
                                        void *out, unsigned long outStride, unsigned long long *used, void *stream)
 {
-    return encode_rgba_batch(bc7_codec(), rgba, frames, frameStride, width, height, rowBytes, compressor, chunkCount, out, outStride, used,
+    return encode_picture_batch(bc7_codec(), rgba_picture(rgba), frames, frameStride, width, height, rowBytes, compressor, chunkCount, out, outStride, used,
                              stream);
 }
 
 unsigned int HapB200BlockEncodeBC7Batch(const void *rgba, unsigned int frames, unsigned long frameStride, unsigned int width,
                                         unsigned int height, unsigned long rowBytes, void *blocks, unsigned long blocksStride, void *stream)
 {
-    return block_encode_rgba_batch(bc7_codec(), rgba, frames, frameStride, width, height, rowBytes, blocks, blocksStride, stream);
+    return block_encode_picture_batch(bc7_codec(), rgba_picture(rgba), frames, frameStride, width, height, rowBytes, blocks, blocksStride, stream);
+}
+
+// ---- NV12 / P010 -> Hap, Hap Alpha, Hap Q, Hap Q Alpha: the picture encoders with a YUV source (yuv_source.cuh) ----------
+
+// the codecs the YUV encoders take (every one with a block compressor that encodes colour) and the layouts and colour spaces
+static bool yuv_args_ok(unsigned layout, unsigned colorSpace, unsigned codec, CodecInfo &ci)
+{
+    return layout <= HapB200YUV_P010 && colorSpace <= HapB200YUV_BT709_Full && codec_info(codec, ci) && codec_encodes(ci) && ci.bc_kind != kBcRgtc1;
+}
+
+static PictureSrc yuv_picture(const void *luma, const void *chroma, unsigned layout, unsigned colorSpace)
+{
+    return {layout == HapB200YUV_P010 ? kSrcP010 : kSrcNv12, luma, chroma, colorSpace};
+}
+
+unsigned int HapB200EncodeYUV(const void *luma, const void *chroma, unsigned int width, unsigned int height, unsigned long pitch,
+                              unsigned int layout, unsigned int colorSpace, unsigned int codec, unsigned int compressor,
+                              unsigned int chunkCount, void *outputBuffer, unsigned long outputBufferBytes, unsigned long *outputBufferBytesUsed)
+{
+    CodecInfo ci;
+    if (!yuv_args_ok(layout, colorSpace, codec, ci)) return HapResult_Bad_Arguments;
+    return encode_picture(ci, yuv_picture(luma, chroma, layout, colorSpace), width, height, pitch, compressor, chunkCount, outputBuffer,
+                          outputBufferBytes, outputBufferBytesUsed);
+}
+
+unsigned int HapB200EncodeYUVBatch(const void *luma, const void *chroma, unsigned int frames, unsigned long frameStride, unsigned int width,
+                                   unsigned int height, unsigned long pitch, unsigned int layout, unsigned int colorSpace, unsigned int codec,
+                                   unsigned int compressor, unsigned int chunkCount, void *out, unsigned long outStride,
+                                   unsigned long long *used, void *stream)
+{
+    CodecInfo ci;
+    if (!yuv_args_ok(layout, colorSpace, codec, ci)) return HapResult_Bad_Arguments;
+    return encode_picture_batch(ci, yuv_picture(luma, chroma, layout, colorSpace), frames, frameStride, width, height, pitch, compressor,
+                                chunkCount, out, outStride, used, stream);
+}
+
+unsigned int HapB200BlockEncodeYUVBatch(const void *luma, const void *chroma, unsigned int frames, unsigned long frameStride,
+                                        unsigned int width, unsigned int height, unsigned long pitch, unsigned int layout,
+                                        unsigned int colorSpace, unsigned int codec, void *blocks, unsigned long blocksStride, void *stream)
+{
+    CodecInfo ci;
+    if (!yuv_args_ok(layout, colorSpace, codec, ci)) return HapResult_Bad_Arguments;
+    return block_encode_picture_batch(ci, yuv_picture(luma, chroma, layout, colorSpace), frames, frameStride, width, height, pitch, blocks,
+                                      blocksStride, stream);
 }
 
 unsigned int HapB200DecodeBatch(const void *in, unsigned int frames, unsigned long inStride, const unsigned long long *inBytes,

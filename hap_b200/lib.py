@@ -12,6 +12,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 HapB200Codec_Hap1, HapB200Codec_Hap5, HapB200Codec_HapY, HapB200Codec_HapM, HapB200Codec_HapA, HapB200Codec_Hap7 = range(6)
 # HapB200Codec_Hap7 ("Hap R", BC7): the codec-taking RGBA encode entry points refuse it with HapResult_Bad_Arguments; the
 # BC7 encoders (encode_rgba_bc7, encode_rgba_bc7_batch, block_encode_bc7_batch) ask for it by name
+HapB200YUV_NV12, HapB200YUV_P010 = range(2)
+HapB200YUV_BT601_Limited, HapB200YUV_BT601_Full, HapB200YUV_BT709_Limited, HapB200YUV_BT709_Full = range(4)
 
 
 def library_path() -> str:
@@ -76,6 +78,12 @@ class HapB200(HapABI):
         L.HapB200BlockEncodeBC7Batch.restype = u
         L.HapB200BlockEncodeBC7Batch.argtypes = [vp, u, ul, u, u, ul, vp, ul, vp]
         L.HapB200BlockEncodeHalfBatch.argtypes = [vp, u, ul, u, u, ul, u, vp, ul, vp]
+        L.HapB200EncodeYUV.restype = u
+        L.HapB200EncodeYUV.argtypes = [vp, vp, u, u, ul, u, u, u, u, u, vp, ul, C.POINTER(ul)]
+        L.HapB200EncodeYUVBatch.restype = u
+        L.HapB200EncodeYUVBatch.argtypes = [vp, vp, u, ul, u, u, ul, u, u, u, u, u, vp, ul, vp, vp]
+        L.HapB200BlockEncodeYUVBatch.restype = u
+        L.HapB200BlockEncodeYUVBatch.argtypes = [vp, vp, u, ul, u, u, ul, u, u, u, vp, ul, vp]
         for name, args in (("RingCreate", [C.c_int, ul, C.POINTER(vp), vp]), ("RingDestroy", [C.c_int, vp]),
                            ("RingOpen", [C.c_int, vp, C.POINTER(vp)]), ("RingClose", [C.c_int, vp]),
                            ("RingAttach", [C.c_int, C.c_int]), ("RingPublish", [C.c_int, vp, u, vp]), ("RingWait", [C.c_int, vp, u, u, vp])):
@@ -269,6 +277,36 @@ class HapB200(HapABI):
     def block_encode_bc7_batch(self, rgba, frames, frame_stride, w, h, blocks, blocks_stride, row_bytes=None, stream=None):
         return int(self.lib.HapB200BlockEncodeBC7Batch(rgba, frames, frame_stride, w, h, row_bytes or 4 * w, blocks, blocks_stride,
                                                        stream))
+
+    # -- NV12 / P010 -> Hap, Hap Alpha, Hap Q, Hap Q Alpha: layout HapB200YUV_*, color_space HapB200YUV_BT*; both planes
+    #    have the row pitch `pitch` (default: width bytes per sample); frames need max_encoded_length_rgba(w, h, codec, chunks)
+    def encode_yuv(self, luma, chroma, w, h, layout, color_space, codec, compressor=1, chunks=1, pitch=None, out=None,
+                   out_capacity=None):
+        """luma, chroma: buffer objects or (addr, nbytes).  Returns (result, frame bytes | used)."""
+        from .abi import _as_ptr
+        laddr, _ = _as_ptr(luma)
+        caddr, _ = _as_ptr(chroma)
+        cap = self.max_encoded_length_rgba(w, h, codec, chunks) if out_capacity is None else out_capacity
+        own = out is None
+        if own:
+            out = bytearray(max(cap, 1))
+        oaddr, _ = _as_ptr(out)
+        used = C.c_ulong(0)
+        r = self.lib.HapB200EncodeYUV(laddr, caddr, w, h, pitch or (2 if layout == HapB200YUV_P010 else 1) * w, layout, color_space,
+                                      codec, compressor, chunks, oaddr, cap, C.byref(used))
+        if r != 0:
+            return int(r), None
+        return 0, (bytes(memoryview(out)[: used.value]) if own else used.value)
+
+    def encode_yuv_batch(self, luma, chroma, frames, frame_stride, w, h, pitch, layout, color_space, codec, compressor, chunks, out,
+                         out_stride, used, stream=None):
+        return int(self.lib.HapB200EncodeYUVBatch(luma, chroma, frames, frame_stride, w, h, pitch, layout, color_space, codec,
+                                                  compressor, chunks, out, out_stride, used, stream))
+
+    def block_encode_yuv_batch(self, luma, chroma, frames, frame_stride, w, h, pitch, layout, color_space, codec, blocks,
+                               blocks_stride, stream=None):
+        return int(self.lib.HapB200BlockEncodeYUVBatch(luma, chroma, frames, frame_stride, w, h, pitch, layout, color_space, codec,
+                                                       blocks, blocks_stride, stream))
 
     # -- delivery rings (include/hap_b200.h): frames written straight into another GPU's memory -----------------
     RING_HANDLE_BYTES = 64

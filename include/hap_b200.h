@@ -251,6 +251,76 @@ unsigned int HapB200BlockEncodeBC7Batch(const void *rgba, unsigned int frames, u
                                         unsigned int width, unsigned int height, unsigned long rowBytes,
                                         void *blocks, unsigned long blocksStride, void *stream);
 
+/* ---- Hap, Hap Alpha, Hap Q, Hap Q Alpha <- NV12 / P010 ----------------------------------------------------------------------
+ * The encoders take the 4:2:0 pictures a video decoder writes (NVDEC surfaces) and convert them to RGBA8 inside the block
+ * encoder, so no RGBA picture is ever written.  Encoding a YUV picture gives exactly the bytes HapB200EncodeRGBA* gives for
+ * the RGBA8 picture the conversion below makes of it.
+ * Planes:
+ *   HapB200YUV_NV12: luma is one byte per pixel; chroma is interleaved Cb, Cr byte pairs, width/2 pairs per row, height/2 rows.
+ *   HapB200YUV_P010: the same shape in little-endian 16-bit words; the sample is word >> 6 (the low 6 bits are ignored).
+ *   Both planes have the same row pitch (bytes), as NVDEC surfaces do.  chroma is a pointer of its own: NVDEC places it at
+ *   pitch * surfaceHeight, not at pitch * height.  In a batch frame f's planes start at luma + f*frameStride and
+ *   chroma + f*frameStride.
+ * Geometry: width and height multiples of 4, width * (bytes per sample) <= pitch <= HAPB200_MAX_ROW_BYTES, at most
+ * HAPB200_MAX_BLOCKS blocks.  The batch entry points take device pointers; luma, chroma, pitch, frameStride, out, outStride,
+ * blocks and blocksStride are 16-byte aligned; a batch may hold any number of frames.
+ * Codecs: HapB200Codec_Hap1, _Hap5, _HapY and _HapM, with A = 255.  HapB200Codec_HapA (the picture has no alpha) and
+ * HapB200Codec_Hap7 (as for every codec-taking encoder) are refused with HapResult_Bad_Arguments, as are an unknown layout
+ * or colour space.  Every argument is checked before anything touches the GPU.  Sizes (HapB200MaxEncodedLengthRGBA),
+ * compressor, chunkCount, HapResult_Buffer_Too_Small and the index, offset-table and chroma-refine options behave exactly
+ * as for HapB200EncodeRGBA*.
+ * The conversion, exactly (n = 8 for NV12, 10 for P010):
+ *   Chroma upsampling: bilinear, MPEG-2 / H.264 / HEVC default siting (chroma_sample_loc_type 0): chroma is co-sited with
+ *   even luma columns and midway between luma rows 2j and 2j+1.  For luma (x, y), i = x/2 and j = y/2 (rounded down); the
+ *   upsampled value in eighths is C8 = sum of wh*wv*C over: vertical weight 3 on row j and 1 on row j-1 (y even) or j+1
+ *   (y odd); horizontal weight 2 on column i (x even), or 1 and 1 on columns i and i+1 (x odd).  Row and column indices are
+ *   clamped to the chroma plane.
+ *   Matrix: the Y'CbCr -> R'G'B' matrix of (Kr, Kb) = BT.601 (0.299, 0.114) or BT.709 (0.2126, 0.0722).  Limited range:
+ *   luma offset 16 * 2^(n-8), luma scale 219 * 2^(n-8), chroma scale 224 * 2^(n-8); full range: luma offset 0, both
+ *   scales 2^n - 1.  Chroma offset 2^(n-1).
+ *   Fixed point: with the row {cy, crR, cbG, crG, cbB, yOff, cOff} of HAPB200_YUV_COEFFICIENTS below (each coefficient
+ *   round(65536 * 255 * matrix entry / scale), the chroma ones divided by 8 more for the eighths; in limited range the NV12
+ *   coefficients are 4 times the P010 ones, so a P010 picture whose samples are 4 times an NV12 picture's converts to the
+ *   same RGBA), Yd = Y - yOff,
+ *   Cb8d = Cb8 - 8*cOff and Cr8d = Cr8 - 8*cOff:
+ *     R = (cy*Yd + crR*Cr8d + 32768) >> 16,  G = (cy*Yd + cbG*Cb8d + crG*Cr8d + 32768) >> 16,  B = (cy*Yd + cbB*Cb8d + 32768) >> 16,
+ *   the shift arithmetic, each result clamped to 0..255 (samples outside the nominal range are not clamped first); A = 255. */
+enum HapB200YUVLayout { HapB200YUV_NV12 = 0, HapB200YUV_P010 = 1 };
+enum HapB200YUVColorSpace {
+    HapB200YUV_BT601_Limited = 0,
+    HapB200YUV_BT601_Full = 1,
+    HapB200YUV_BT709_Limited = 2,
+    HapB200YUV_BT709_Full = 3
+};
+/* row layout * 4 + colorSpace: {cy, crR, cbG, crG, cbB, yOff, cOff} */
+#define HAPB200_YUV_COEFFICIENTS                                                                                           \
+    {                                                                                                                      \
+        {76308, 13076, -3208, -6660, 16524, 16, 128},  /* NV12 BT.601 limited */                                           \
+        {65536, 11485, -2819, -5850, 14516, 0, 128},   /* NV12 BT.601 full    */                                           \
+        {76308, 14688, -1748, -4364, 17304, 16, 128},  /* NV12 BT.709 limited */                                           \
+        {65536, 12901, -1535, -3835, 15201, 0, 128},   /* NV12 BT.709 full    */                                           \
+        {19077, 3269, -802, -1665, 4131, 64, 512},     /* P010 BT.601 limited */                                           \
+        {16336, 2863, -703, -1458, 3618, 0, 512},      /* P010 BT.601 full    */                                           \
+        {19077, 3672, -437, -1091, 4326, 64, 512},     /* P010 BT.709 limited */                                           \
+        {16336, 3216, -383, -956, 3789, 0, 512}        /* P010 BT.709 full    */                                           \
+    }
+
+/* one picture (host or device pointers) -> one Hap frame */
+unsigned int HapB200EncodeYUV(const void *luma, const void *chroma, unsigned int width, unsigned int height,
+                              unsigned long pitch, unsigned int layout, unsigned int colorSpace, unsigned int codec,
+                              unsigned int compressor, unsigned int chunkCount,
+                              void *outputBuffer, unsigned long outputBufferBytes, unsigned long *outputBufferBytesUsed);
+/* frames x picture (device) -> frames x Hap frame at out + f*outStride, encoded length in used[f] (device) */
+unsigned int HapB200EncodeYUVBatch(const void *luma, const void *chroma, unsigned int frames, unsigned long frameStride,
+                                   unsigned int width, unsigned int height, unsigned long pitch, unsigned int layout,
+                                   unsigned int colorSpace, unsigned int codec, unsigned int compressor, unsigned int chunkCount,
+                                   void *out, unsigned long outStride, unsigned long long *used, void *stream);
+/* frames x picture (device) -> bare textures, as HapB200BlockEncodeBatch (HapM: the RGTC1 plane at blocks + HapB200TextureBytes(.., 0)) */
+unsigned int HapB200BlockEncodeYUVBatch(const void *luma, const void *chroma, unsigned int frames, unsigned long frameStride,
+                                        unsigned int width, unsigned int height, unsigned long pitch, unsigned int layout,
+                                        unsigned int colorSpace, unsigned int codec, void *blocks, unsigned long blocksStride,
+                                        void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1,0 +1,24 @@
+"""The NV12 / P010 instantiations of the block encode kernel (bc_encode_kernel with a YUV source) under the fiber SIMT
+emulator at odd block widths, wide pitches, strided frames, wide block strides and an NVDEC-style chroma plane
+(tests/emu/test_yuv_emu.cc).  Each block must equal the per-block encoder applied to the reference conversion of its
+pixels.  Once plainly and once under AddressSanitizer with exact-size planes."""
+import os
+import subprocess
+
+import pytest
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+BUILD = os.path.join(ROOT, "tests", "emu", "_build")
+INC = ["-I", os.path.join(ROOT, "hap_b200", "csrc"), "-I", os.path.join(ROOT, "tests", "emu")]
+
+
+@pytest.mark.parametrize("asan", [False, True])
+def test_yuv_block_encode_kernels_emulated(asan):
+    os.makedirs(BUILD, exist_ok=True)
+    exe = os.path.join(BUILD, "test_yuv_emu" + ("_asan" if asan else ""))
+    subprocess.run(["g++", "-std=c++17", "-O1", "-g", "-w"] + (["-fsanitize=address"] if asan else []) + INC +
+                   [os.path.join(ROOT, "tests", "emu", "test_yuv_emu.cc"), "-ldl", "-lm", "-o", exe], check=True)
+    env = dict(os.environ, ASAN_OPTIONS="detect_stack_use_after_return=0:detect_leaks=0")
+    p = subprocess.run([exe], capture_output=True, text=True, timeout=900, env=env)
+    assert p.returncode == 0, p.stdout[-2000:] + p.stderr[-4000:]
+    assert " 0 failures" in p.stdout

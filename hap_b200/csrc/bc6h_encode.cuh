@@ -1,5 +1,5 @@
-// hap_b200/csrc/bc6h_encode.cuh -- K1-K4 family: RGBA16F pictures -> BPTC / BC6H blocks (UF16 or SF16, "Hap HDR"),
-// bc6h_encode_kernel.
+// hap_b200/csrc/bc6h_encode.cuh -- K1-K4 family: RGBA16F (or HDR10 P010) pictures -> BPTC / BC6H blocks (UF16 or SF16,
+// "Hap HDR"), bc6h_encode_kernel.
 //
 // Shape as the other block encoders (bc_encode.cuh): one thread per 4x4 block, kBcThreads per CTA, frames on blockIdx.y in
 // slices of kBcFramesPerLaunch.  A block row of RGBA16F is 32 bytes, read as two 128-bit loads, so a warp reads 1 KiB
@@ -477,23 +477,32 @@ HAP_HD uint64_t bc6h_encode_block(const uint32_t px[32], bool sgn, uint32_t out[
 }
 
 // grid = (bc_ctas, frames), G as for bc_encode_kernel with 8 bytes per pixel (row_bytes >= 8 * width, out_stride >= 16 per
-// block).  is_signed: SF16, else UF16.
+// block).  is_signed: SF16, else UF16.  SRC (BcSource): kSrcRgbaHalf reads `rgba` as RGBA16F rows; kSrcP010Pq reads it as
+// the luma plane of an HDR10 P010 picture and P.m.chroma as its chroma plane, both frame_bytes apart per frame and rows
+// row_bytes apart, and converts them to RGBA16F (yuv_source.cuh) before the search.  P comes last so that the parameters of
+// the RGBA16F instantiation keep their offsets.
+template <int SRC = kSrcRgbaHalf>
 __global__ void __launch_bounds__(kBcThreads) bc6h_encode_kernel(const uint8_t *__restrict__ rgba, BcGeom G, uint8_t *__restrict__ out,
-                                                                 uint32_t is_signed)
+                                                                 uint32_t is_signed, YuvPqSrc P = YuvPqSrc())
 {
     const uint32_t nblocks = G.blocks_x * G.blocks_y;
     const uint32_t bi = blockIdx.x * kBcThreads + threadIdx.x;
     if (bi >= nblocks) return;
     uint32_t by = __umulhi(bi, G.inv_blocks_x), bx = bi - by * G.blocks_x;  // the estimate is exact or one short
     if (bx >= G.blocks_x) { by++; bx -= G.blocks_x; }
-    const uint8_t *src = rgba + (uint64_t)blockIdx.y * G.frame_bytes + (uint64_t)(4 * by) * G.row_bytes + 32u * bx;
     uint32_t px[32];
+    if (SRC == kSrcRgbaHalf) {
+        const uint8_t *src = rgba + (uint64_t)blockIdx.y * G.frame_bytes + (uint64_t)(4 * by) * G.row_bytes + 32u * bx;
 #pragma unroll
-    for (int row = 0; row < 4; row++) {
-        const uint4 *s = reinterpret_cast<const uint4 *>(src + (uint64_t)row * G.row_bytes);
-        const uint4 v0 = s[0], v1 = s[1];
-        px[8 * row] = v0.x; px[8 * row + 1] = v0.y; px[8 * row + 2] = v0.z; px[8 * row + 3] = v0.w;
-        px[8 * row + 4] = v1.x; px[8 * row + 5] = v1.y; px[8 * row + 6] = v1.z; px[8 * row + 7] = v1.w;
+        for (int row = 0; row < 4; row++) {
+            const uint4 *s = reinterpret_cast<const uint4 *>(src + (uint64_t)row * G.row_bytes);
+            const uint4 v0 = s[0], v1 = s[1];
+            px[8 * row] = v0.x; px[8 * row + 1] = v0.y; px[8 * row + 2] = v0.z; px[8 * row + 3] = v0.w;
+            px[8 * row + 4] = v1.x; px[8 * row + 5] = v1.y; px[8 * row + 6] = v1.z; px[8 * row + 7] = v1.w;
+        }
+    } else {
+        const uint64_t f = (uint64_t)blockIdx.y * G.frame_bytes;
+        load_block_yuv_pq(rgba + f, P.m.chroma + f, G.row_bytes, bx, by, G.blocks_x, G.blocks_y, P, px);
     }
     uint32_t w[4];
     bc6h_encode_block(px, is_signed != 0u, w);

@@ -21,6 +21,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <map>
 #include <mutex>
 #include <vector>
 
@@ -389,15 +390,79 @@ uint32_t launch_block_encode(const uint8_t *rgba, uint32_t frames, uint64_t fram
     return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
 }
 
-// RGBA16F pictures -> BC6H blocks (Hap HDR), SF16 when is_signed, else UF16.  One launch per kBcFramesPerLaunch frames.
-uint32_t launch_bc6h_encode(const uint8_t *rgba, uint32_t frames, uint64_t frame_stride, uint32_t width, uint32_t height, uint64_t row_bytes,
+// The PQ tables of the HDR10 encoders: T of include/hap_b200.h per (device, unitNits), built on the host (yuv_pq_table) and
+// uploaded by the first call that needs it, which waits for the copy; 8 KiB each, kept for the life of the process, so later
+// calls (batches among them) find it without touching the host.  nullptr when the upload fails.
+const uint16_t *pq_table(uint32_t unit_nits)
+{
+    static std::mutex mu;
+    static std::map<uint32_t, uint16_t *> tables[kMaxDevices];
+    std::lock_guard<std::mutex> l(mu);
+    std::map<uint32_t, uint16_t *> &mine = tables[t_device];
+    const auto it = mine.find(unit_nits);
+    if (it != mine.end()) return it->second;
+    std::vector<uint16_t> host(4096);
+    yuv_pq_table(unit_nits, host.data());
+    void *d = nullptr;
+    cudaStream_t s = nullptr;
+    bool ok = cudaMalloc(&d, 4096 * sizeof(uint16_t)) == cudaSuccess && cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking) == cudaSuccess;
+    ok = ok && cudaMemcpyAsync(d, host.data(), 4096 * sizeof(uint16_t), cudaMemcpyHostToDevice, s) == cudaSuccess;
+    ok = ok && cudaStreamSynchronize(s) == cudaSuccess;
+    if (s) cudaStreamDestroy(s);
+    if (!ok) {
+        cudaGetLastError();
+        if (d) cudaFree(d);
+        return nullptr;
+    }
+    return mine[unit_nits] = (uint16_t *)d;
+}
+
+// The picture an encoder reads: an RGBA8 picture (kSrcRgba8), the luma and chroma planes of an NV12 / P010 picture
+// (kSrcNv12 / kSrcP010, yuv_source.cuh), an RGBA16F picture (kSrcRgbaHalf) or an HDR10 P010 picture (kSrcP010Pq).  Rows of
+// both planes are `pitch` bytes apart.
+struct PictureSrc {
+    int kind;                 // BcSource
+    const void *pixels;       // the RGBA8 / RGBA16F picture, or the luma plane
+    const void *chroma;       // the interleaved CbCr plane
+    unsigned color_space;     // HapB200YUVColorSpace
+    unsigned unit_nits = 0;   // kSrcP010Pq: the luminance of 1.0
+    uint64_t sample_bytes() const   // per pixel of a luma / RGBA row
+    {
+        return kind == kSrcRgba8 ? 4 : kind == kSrcRgbaHalf ? 8 : kind == kSrcNv12 ? 1 : 2;
+    }
+    uint32_t planes() const { return kind == kSrcRgba8 || kind == kSrcRgbaHalf ? 1 : 2; }
+    YuvSrc yuv() const
+    {
+        return kind == kSrcNv12 || kind == kSrcP010 ? yuv_src(kind - kSrcNv12, color_space, (const uint8_t *)chroma) : YuvSrc();
+    }
+};
+PictureSrc rgba_picture(const void *rgba) { return {kSrcRgba8, rgba, nullptr, 0}; }
+PictureSrc rgba_half_picture(const void *rgba) { return {kSrcRgbaHalf, rgba, nullptr, 0}; }
+
+// RGBA16F / HDR10 P010 pictures (p: kSrcRgbaHalf / kSrcP010Pq, its planes frame_stride apart) -> BC6H blocks (Hap HDR), SF16
+// when is_signed, else UF16.  One launch per kBcFramesPerLaunch frames.
+uint32_t launch_bc6h_encode(const PictureSrc &p, uint32_t frames, uint64_t frame_stride, uint32_t width, uint32_t height, uint64_t row_bytes,
                             uint8_t *blocks, uint64_t blocks_stride, bool is_signed, cudaStream_t st)
 {
     const BcGeom g = bc_encode_geom(width, height, (uint32_t)row_bytes, frame_stride, blocks_stride, 0);   // (rgba_geometry_ok: row_bytes < 2^32)
+    YuvPqSrc pq = YuvPqSrc();
+    if (p.kind == kSrcP010Pq) {
+        const uint16_t *table = pq_table(p.unit_nits);
+        if (!table) return HapResult_Internal_Error;
+        pq = yuv_pq_src(p.color_space, (const uint8_t *)p.chroma, table);
+    }
+    const uint8_t *src = (const uint8_t *)p.pixels;
     for (uint32_t f0 = 0; f0 < frames; f0 += kBcFramesPerLaunch) {
         const dim3 grid(bc_ctas(g.blocks_x, g.blocks_y), frames - f0 < kBcFramesPerLaunch ? frames - f0 : kBcFramesPerLaunch);
-        HAP_KLAUNCH(kStBcEncode, bc6h_encode_kernel, grid, dim3(kBcThreads), 0, st, rgba + f0 * g.frame_bytes, g, blocks + f0 * g.out_stride,
-                    is_signed ? 1u : 0u);
+        if (p.kind == kSrcP010Pq) {
+            YuvPqSrc y = pq;
+            y.m.chroma += f0 * g.frame_bytes;
+            HAP_KLAUNCH(kStBcEncode, bc6h_encode_kernel<kSrcP010Pq>, grid, dim3(kBcThreads), 0, st, src + f0 * g.frame_bytes, g,
+                        blocks + f0 * g.out_stride, is_signed ? 1u : 0u, y);
+        } else {
+            HAP_KLAUNCH(kStBcEncode, bc6h_encode_kernel<>, grid, dim3(kBcThreads), 0, st, src + f0 * g.frame_bytes, g, blocks + f0 * g.out_stride,
+                        is_signed ? 1u : 0u, pq);
+        }
     }
     return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
 }
@@ -1139,19 +1204,6 @@ unsigned long HapB200MaxEncodedLengthRGBA(unsigned int width, unsigned int heigh
     return max_encoded_length_rgba(width, height, ci, chunkCount);
 }
 
-// The picture an encoder reads: an RGBA8 picture (kSrcRgba8), or the luma and chroma planes of an NV12 / P010 picture
-// (kSrcNv12 / kSrcP010, yuv_source.cuh).  Rows of both planes are `pitch` bytes apart.
-struct PictureSrc {
-    int kind;                 // BcSource
-    const void *pixels;       // the RGBA8 picture, or the luma plane
-    const void *chroma;       // the interleaved CbCr plane
-    unsigned color_space;     // HapB200YUVColorSpace
-    uint64_t sample_bytes() const { return kind == kSrcRgba8 ? 4 : kind == kSrcP010 ? 2 : 1; }   // per pixel of a luma / RGBA row
-    uint32_t planes() const { return kind == kSrcRgba8 ? 1 : 2; }
-    YuvSrc yuv() const { return kind == kSrcRgba8 ? YuvSrc() : yuv_src(kind - kSrcNv12, color_space, (const uint8_t *)chroma); }
-};
-PictureSrc rgba_picture(const void *rgba) { return {kSrcRgba8, rgba, nullptr, 0}; }
-
 // width x height NV12 (bpp 1) / P010 (bpp 2) planes with one pitch: the chroma plane's rows hold as many bytes as luma's.
 // aligned: the batch entry points' rules besides (16-byte aligned pitch, planes and frame stride).
 bool yuv_geometry_ok(const void *luma, const void *chroma, unsigned width, unsigned height, unsigned long pitch, unsigned long frameStride,
@@ -1162,7 +1214,7 @@ bool yuv_geometry_ok(const void *luma, const void *chroma, unsigned width, unsig
 
 bool picture_geometry_ok(const PictureSrc &p, unsigned width, unsigned height, unsigned long pitch, unsigned long frameStride, bool aligned)
 {
-    if (p.kind == kSrcRgba8) return rgba_geometry_ok(p.pixels, width, height, pitch, frameStride, aligned);
+    if (p.planes() == 1) return rgba_geometry_ok(p.pixels, width, height, pitch, frameStride, aligned, p.sample_bytes());
     return yuv_geometry_ok(p.pixels, p.chroma, width, height, pitch, frameStride, aligned, p.sample_bytes());
 }
 
@@ -1200,23 +1252,21 @@ static unsigned encode_picture_batch(const CodecInfo &ci, const PictureSrc &p, u
     });
 }
 
-// One picture in host or device memory: its planes are copied into tight device scratch (rows align16(row bytes) apart,
-// chroma after luma) and encoded as a batch of one.
-static unsigned encode_picture(const CodecInfo &ci, const PictureSrc &p, unsigned width, unsigned height, unsigned long pitch, unsigned compressor,
-                               unsigned chunkCount, void *outputBuffer, unsigned long outputBufferBytes, unsigned long *outputBufferBytesUsed)
+// One picture in host or device memory, its arguments checked: its planes are copied into tight device scratch (rows
+// align16(row bytes) apart, chroma after luma) and encoded as a batch of one by
+// batch(device picture, its frame stride, its pitch, out, outStride, used, stream).  cap: the frame's size bound.
+extern "C++" {   // (a template, inside the C ABI block)
+template <class Batch>
+static unsigned encode_one_picture(const PictureSrc &p, unsigned width, unsigned height, unsigned long pitch, unsigned long cap,
+                                   void *outputBuffer, unsigned long outputBufferBytes, unsigned long *outputBufferBytesUsed, Batch &&batch)
 {
-    if (!outputBuffer || !outputBufferBytesUsed || chunkCount == 0 || !picture_geometry_ok(p, width, height, pitch, 0, false) ||
-        (compressor != HapCompressorNone && compressor != HapCompressorSnappy))
-        return HapResult_Bad_Arguments;
-    const unsigned long cap = max_encoded_length_rgba(width, height, ci, chunkCount);
-    if (outputBufferBytes < cap) return HapResult_Buffer_Too_Small;
     HAP_ENTER(p.pixels, outputBuffer);
     CallStream call(!is_device(p.pixels) && !is_device(p.chroma) && !is_device(outputBuffer));
     cudaStream_t st = call.st;
     DevBuf img(st), frame(st), used(st);
-    const uint64_t row = p.sample_bytes() * width, tight = align16(row);   // (RGBA8: tight = row, width is a multiple of 4)
+    const uint64_t row = p.sample_bytes() * width, tight = align16(row);   // (RGBA8, RGBA16F: tight = row, width is a multiple of 4)
     const uint64_t luma_bytes = tight * height, plane_bytes = luma_bytes + (p.planes() == 2 ? tight * (height / 2) : 0);
-    if (!img.alloc(plane_bytes) || !frame.alloc(cap) || !used.alloc(32)) { cudaGetLastError(); return HapResult_Internal_Error; }
+    if (!img.alloc(plane_bytes) || !frame.alloc(align16(cap)) || !used.alloc(32)) { cudaGetLastError(); return HapResult_Internal_Error; }
     PictureSrc dev = p;
     dev.pixels = img.p;
     if (cudaMemcpy2DAsync(img.p, tight, p.pixels, pitch, row, height, cudaMemcpyDefault, st) != cudaSuccess) { cudaGetLastError(); return HapResult_Internal_Error; }
@@ -1227,8 +1277,7 @@ static unsigned encode_picture(const CodecInfo &ci, const PictureSrc &p, unsigne
             return HapResult_Internal_Error;
         }
     }
-    uint32_t r = encode_picture_batch(ci, dev, 1, align16(plane_bytes), width, height, tight, compressor, chunkCount, frame.p, cap,
-                                      used.as<unsigned long long>(), st);
+    uint32_t r = batch(dev, align16(plane_bytes), tight, frame.p, align16(cap), used.as<unsigned long long>(), st);
     if (r != HapResult_No_Error) return r;
     unsigned long long total = 0;
     if (cudaMemcpyAsync(&total, used.p, sizeof total, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess ||
@@ -1236,6 +1285,23 @@ static unsigned encode_picture(const CodecInfo &ci, const PictureSrc &p, unsigne
         cudaStreamSynchronize(st) != cudaSuccess) { cudaGetLastError(); return HapResult_Internal_Error; }
     *outputBufferBytesUsed = (unsigned long)total;
     return HapResult_No_Error;
+}
+}  // extern "C++"
+
+static unsigned encode_picture(const CodecInfo &ci, const PictureSrc &p, unsigned width, unsigned height, unsigned long pitch, unsigned compressor,
+                               unsigned chunkCount, void *outputBuffer, unsigned long outputBufferBytes, unsigned long *outputBufferBytesUsed)
+{
+    if (!outputBuffer || !outputBufferBytesUsed || chunkCount == 0 || !picture_geometry_ok(p, width, height, pitch, 0, false) ||
+        (compressor != HapCompressorNone && compressor != HapCompressorSnappy))
+        return HapResult_Bad_Arguments;
+    const unsigned long cap = max_encoded_length_rgba(width, height, ci, chunkCount);
+    if (outputBufferBytes < cap) return HapResult_Buffer_Too_Small;
+    return encode_one_picture(p, width, height, pitch, cap, outputBuffer, outputBufferBytes, outputBufferBytesUsed,
+                              [&](const PictureSrc &dev, uint64_t fstride, uint64_t tight, void *out, uint64_t ostride, unsigned long long *used,
+                                  cudaStream_t st) {
+                                  return encode_picture_batch(ci, dev, 1, fstride, width, height, tight, compressor, chunkCount, out, ostride,
+                                                              used, st);
+                              });
 }
 
 unsigned int HapB200BlockEncodeBatch(const void *rgba, unsigned int frames, unsigned long frameStride, unsigned int width,
@@ -1528,66 +1594,122 @@ static unsigned long bc6h_max_encoded_length(unsigned width, unsigned height, un
     return HapMaxEncodedLength(1, &len, &fmt, &chunks);
 }
 
+// The BC6H encoders of an RGBA16F picture (kSrcRgbaHalf) and of an HDR10 P010 picture (kSrcP010Pq)
+static unsigned block_encode_bc6h_batch(const PictureSrc &p, unsigned frames, unsigned long frameStride, unsigned width, unsigned height,
+                                        unsigned long pitch, unsigned textureFormat, void *blocks, unsigned long blocksStride, void *stream)
+{
+    if (!blocks || frames == 0 || !is_bc6h_format(textureFormat) || !picture_geometry_ok(p, width, height, pitch, frameStride, true) ||
+        ((uintptr_t)blocks | blocksStride) % 16)
+        return HapResult_Bad_Arguments;
+    HAP_ENTER(p.pixels, blocks);
+    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
+        return launch_bc6h_encode(p, frames, frameStride, width, height, pitch, (uint8_t *)blocks, blocksStride,
+                                  textureFormat == HapFmt_RGB_BPTC_SFLOAT, st);
+    });
+}
+
+static unsigned encode_bc6h_batch(const PictureSrc &p, unsigned frames, unsigned long frameStride, unsigned width, unsigned height,
+                                  unsigned long pitch, unsigned textureFormat, unsigned compressor, unsigned chunkCount, void *out,
+                                  unsigned long outStride, unsigned long long *used, void *stream)
+{
+    if (!out || !used || frames == 0 || chunkCount == 0 || !is_bc6h_format(textureFormat) ||
+        !picture_geometry_ok(p, width, height, pitch, frameStride, true) || ((uintptr_t)out | outStride) % 16 ||
+        (compressor != HapCompressorNone && compressor != HapCompressorSnappy))
+        return HapResult_Bad_Arguments;
+    if (outStride < bc6h_max_encoded_length(width, height, textureFormat, chunkCount)) return HapResult_Buffer_Too_Small;
+    HAP_ENTER(p.pixels, out);
+    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
+        const uint64_t t[2] = {(uint64_t)(width / 4) * (height / 4) * 16, 0};
+        const uint32_t fmt[2] = {textureFormat, 0};
+        return encode_frames_from_blocks(frames, 1, t, fmt, compressor, chunkCount, (uint8_t *)out, outStride, used, st,
+                                         [&](uint8_t *tex, uint64_t stride) {
+                                             return launch_bc6h_encode(p, frames, frameStride, width, height, pitch, tex, stride,
+                                                                       textureFormat == HapFmt_RGB_BPTC_SFLOAT, st);
+                                         });
+    });
+}
+
+static unsigned encode_bc6h_picture(const PictureSrc &p, unsigned width, unsigned height, unsigned long pitch, unsigned textureFormat,
+                                    unsigned compressor, unsigned chunkCount, void *outputBuffer, unsigned long outputBufferBytes,
+                                    unsigned long *outputBufferBytesUsed)
+{
+    if (!outputBuffer || !outputBufferBytesUsed || chunkCount == 0 || !is_bc6h_format(textureFormat) ||
+        !picture_geometry_ok(p, width, height, pitch, 0, false) || (compressor != HapCompressorNone && compressor != HapCompressorSnappy))
+        return HapResult_Bad_Arguments;
+    const unsigned long cap = bc6h_max_encoded_length(width, height, textureFormat, chunkCount);
+    if (outputBufferBytes < cap) return HapResult_Buffer_Too_Small;
+    return encode_one_picture(p, width, height, pitch, cap, outputBuffer, outputBufferBytes, outputBufferBytesUsed,
+                              [&](const PictureSrc &dev, uint64_t fstride, uint64_t tight, void *out, uint64_t ostride, unsigned long long *used,
+                                  cudaStream_t st) {
+                                  return encode_bc6h_batch(dev, 1, fstride, width, height, tight, textureFormat, compressor, chunkCount, out,
+                                                           ostride, used, st);
+                              });
+}
+
 unsigned int HapB200BlockEncodeHalfBatch(const void *rgbaHalf, unsigned int frames, unsigned long frameStride, unsigned int width,
                                          unsigned int height, unsigned long rowBytes, unsigned int textureFormat, void *blocks,
                                          unsigned long blocksStride, void *stream)
 {
-    if (!blocks || frames == 0 || !is_bc6h_format(textureFormat) || !rgba_geometry_ok(rgbaHalf, width, height, rowBytes, frameStride, true, 8) ||
-        ((uintptr_t)blocks | blocksStride) % 16)
-        return HapResult_Bad_Arguments;
-    HAP_ENTER(rgbaHalf, blocks);
-    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
-        return launch_bc6h_encode((const uint8_t *)rgbaHalf, frames, frameStride, width, height, rowBytes, (uint8_t *)blocks, blocksStride,
-                                  textureFormat == HapFmt_RGB_BPTC_SFLOAT, st);
-    });
+    return block_encode_bc6h_batch(rgba_half_picture(rgbaHalf), frames, frameStride, width, height, rowBytes, textureFormat, blocks,
+                                   blocksStride, stream);
 }
 
 unsigned int HapB200EncodeRGBAHalfBatch(const void *rgbaHalf, unsigned int frames, unsigned long frameStride, unsigned int width,
                                         unsigned int height, unsigned long rowBytes, unsigned int textureFormat, unsigned int compressor,
                                         unsigned int chunkCount, void *out, unsigned long outStride, unsigned long long *used, void *stream)
 {
-    if (!out || !used || frames == 0 || chunkCount == 0 || !is_bc6h_format(textureFormat) ||
-        !rgba_geometry_ok(rgbaHalf, width, height, rowBytes, frameStride, true, 8) || ((uintptr_t)out | outStride) % 16 ||
-        (compressor != HapCompressorNone && compressor != HapCompressorSnappy))
-        return HapResult_Bad_Arguments;
-    if (outStride < bc6h_max_encoded_length(width, height, textureFormat, chunkCount)) return HapResult_Buffer_Too_Small;
-    HAP_ENTER(rgbaHalf, out);
-    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
-        const uint64_t t[2] = {(uint64_t)(width / 4) * (height / 4) * 16, 0};
-        const uint32_t fmt[2] = {textureFormat, 0};
-        return encode_frames_from_blocks(frames, 1, t, fmt, compressor, chunkCount, (uint8_t *)out, outStride, used, st,
-                                         [&](uint8_t *tex, uint64_t stride) {
-                                             return launch_bc6h_encode((const uint8_t *)rgbaHalf, frames, frameStride, width, height, rowBytes,
-                                                                       tex, stride, textureFormat == HapFmt_RGB_BPTC_SFLOAT, st);
-                                         });
-    });
+    return encode_bc6h_batch(rgba_half_picture(rgbaHalf), frames, frameStride, width, height, rowBytes, textureFormat, compressor, chunkCount,
+                             out, outStride, used, stream);
 }
 
 unsigned int HapB200EncodeRGBAHalf(const void *rgbaHalf, unsigned int width, unsigned int height, unsigned long rowBytes,
                                    unsigned int textureFormat, unsigned int compressor, unsigned int chunkCount, void *outputBuffer,
                                    unsigned long outputBufferBytes, unsigned long *outputBufferBytesUsed)
 {
-    if (!outputBuffer || !outputBufferBytesUsed || chunkCount == 0 || !is_bc6h_format(textureFormat) ||
-        !rgba_geometry_ok(rgbaHalf, width, height, rowBytes, 0, false, 8) || (compressor != HapCompressorNone && compressor != HapCompressorSnappy))
-        return HapResult_Bad_Arguments;
-    const unsigned long cap = bc6h_max_encoded_length(width, height, textureFormat, chunkCount);
-    if (outputBufferBytes < cap) return HapResult_Buffer_Too_Small;
-    HAP_ENTER(rgbaHalf, outputBuffer);
-    CallStream call(!is_device(rgbaHalf) && !is_device(outputBuffer));
-    cudaStream_t st = call.st;
-    DevBuf img(st), frame(st), used(st);
-    const uint64_t tight = 8ull * width;
-    if (!img.alloc(tight * height) || !frame.alloc(align16(cap)) || !used.alloc(32)) { cudaGetLastError(); return HapResult_Internal_Error; }
-    if (cudaMemcpy2DAsync(img.p, tight, rgbaHalf, rowBytes, tight, height, cudaMemcpyDefault, st) != cudaSuccess) { cudaGetLastError(); return HapResult_Internal_Error; }
-    uint32_t r = HapB200EncodeRGBAHalfBatch(img.p, 1, align16(tight * height), width, height, tight, textureFormat, compressor, chunkCount,
-                                            frame.p, align16(cap), used.as<unsigned long long>(), st);
-    if (r != HapResult_No_Error) return r;
-    unsigned long long total = 0;
-    if (cudaMemcpyAsync(&total, used.p, sizeof total, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess ||
-        total > outputBufferBytes || cudaMemcpyAsync(outputBuffer, frame.p, total, cudaMemcpyDefault, st) != cudaSuccess ||
-        cudaStreamSynchronize(st) != cudaSuccess) { cudaGetLastError(); return HapResult_Internal_Error; }
-    *outputBufferBytesUsed = (unsigned long)total;
-    return HapResult_No_Error;
+    return encode_bc6h_picture(rgba_half_picture(rgbaHalf), width, height, rowBytes, textureFormat, compressor, chunkCount, outputBuffer,
+                               outputBufferBytes, outputBufferBytesUsed);
+}
+
+// ---- Hap HDR encoding from HDR10: P010, BT.2020, PQ -> BC6H, the BC6H encoders with the kSrcP010Pq source (yuv_source.cuh) ----
+
+// HapB200YUV_BT2020_Limited or _Full, and a unitNits of 1 .. 10000 cd/m2
+static bool yuv_pq_args_ok(unsigned colorSpace, unsigned unitNits)
+{
+    return (colorSpace == HapB200YUV_BT2020_Limited || colorSpace == HapB200YUV_BT2020_Full) && unitNits >= 1 && unitNits <= 10000;
+}
+
+static PictureSrc yuv_pq_picture(const void *luma, const void *chroma, unsigned colorSpace, unsigned unitNits)
+{
+    return {kSrcP010Pq, luma, chroma, colorSpace, unitNits};
+}
+
+unsigned int HapB200EncodeYUVPQ(const void *luma, const void *chroma, unsigned int width, unsigned int height, unsigned long pitch,
+                                unsigned int colorSpace, unsigned int unitNits, unsigned int textureFormat, unsigned int compressor,
+                                unsigned int chunkCount, void *outputBuffer, unsigned long outputBufferBytes, unsigned long *outputBufferBytesUsed)
+{
+    if (!yuv_pq_args_ok(colorSpace, unitNits)) return HapResult_Bad_Arguments;
+    return encode_bc6h_picture(yuv_pq_picture(luma, chroma, colorSpace, unitNits), width, height, pitch, textureFormat, compressor, chunkCount,
+                               outputBuffer, outputBufferBytes, outputBufferBytesUsed);
+}
+
+unsigned int HapB200EncodeYUVPQBatch(const void *luma, const void *chroma, unsigned int frames, unsigned long frameStride, unsigned int width,
+                                     unsigned int height, unsigned long pitch, unsigned int colorSpace, unsigned int unitNits,
+                                     unsigned int textureFormat, unsigned int compressor, unsigned int chunkCount, void *out,
+                                     unsigned long outStride, unsigned long long *used, void *stream)
+{
+    if (!yuv_pq_args_ok(colorSpace, unitNits)) return HapResult_Bad_Arguments;
+    return encode_bc6h_batch(yuv_pq_picture(luma, chroma, colorSpace, unitNits), frames, frameStride, width, height, pitch, textureFormat,
+                             compressor, chunkCount, out, outStride, used, stream);
+}
+
+unsigned int HapB200BlockEncodeYUVPQBatch(const void *luma, const void *chroma, unsigned int frames, unsigned long frameStride,
+                                          unsigned int width, unsigned int height, unsigned long pitch, unsigned int colorSpace,
+                                          unsigned int unitNits, unsigned int textureFormat, void *blocks, unsigned long blocksStride,
+                                          void *stream)
+{
+    if (!yuv_pq_args_ok(colorSpace, unitNits)) return HapResult_Bad_Arguments;
+    return block_encode_bc6h_batch(yuv_pq_picture(luma, chroma, colorSpace, unitNits), frames, frameStride, width, height, pitch,
+                                   textureFormat, blocks, blocksStride, stream);
 }
 
 // ---- include/hap_mov.h: QuickTime sample tables around Hap frames (host code only) -------------------------

@@ -14,6 +14,8 @@ HapB200Codec_Hap1, HapB200Codec_Hap5, HapB200Codec_HapY, HapB200Codec_HapM, HapB
 # BC7 encoders (encode_rgba_bc7, encode_rgba_bc7_batch, block_encode_bc7_batch) ask for it by name
 HapB200YUV_NV12, HapB200YUV_P010 = range(2)
 HapB200YUV_BT601_Limited, HapB200YUV_BT601_Full, HapB200YUV_BT709_Limited, HapB200YUV_BT709_Full = range(4)
+# BT.2020: taken only by the HDR10 encoders (encode_yuv_pq, encode_yuv_pq_batch, block_encode_yuv_pq_batch)
+HapB200YUV_BT2020_Limited, HapB200YUV_BT2020_Full = 4, 5
 
 
 def library_path() -> str:
@@ -84,6 +86,12 @@ class HapB200(HapABI):
         L.HapB200EncodeYUVBatch.argtypes = [vp, vp, u, ul, u, u, ul, u, u, u, u, u, vp, ul, vp, vp]
         L.HapB200BlockEncodeYUVBatch.restype = u
         L.HapB200BlockEncodeYUVBatch.argtypes = [vp, vp, u, ul, u, u, ul, u, u, u, vp, ul, vp]
+        L.HapB200EncodeYUVPQ.restype = u
+        L.HapB200EncodeYUVPQ.argtypes = [vp, vp, u, u, ul, u, u, u, u, u, vp, ul, C.POINTER(ul)]
+        L.HapB200EncodeYUVPQBatch.restype = u
+        L.HapB200EncodeYUVPQBatch.argtypes = [vp, vp, u, ul, u, u, ul, u, u, u, u, u, vp, ul, vp, vp]
+        L.HapB200BlockEncodeYUVPQBatch.restype = u
+        L.HapB200BlockEncodeYUVPQBatch.argtypes = [vp, vp, u, ul, u, u, ul, u, u, u, vp, ul, vp]
         for name, args in (("RingCreate", [C.c_int, ul, C.POINTER(vp), vp]), ("RingDestroy", [C.c_int, vp]),
                            ("RingOpen", [C.c_int, vp, C.POINTER(vp)]), ("RingClose", [C.c_int, vp]),
                            ("RingAttach", [C.c_int, C.c_int]), ("RingPublish", [C.c_int, vp, u, vp]), ("RingWait", [C.c_int, vp, u, u, vp])):
@@ -307,6 +315,37 @@ class HapB200(HapABI):
                                blocks_stride, stream=None):
         return int(self.lib.HapB200BlockEncodeYUVBatch(luma, chroma, frames, frame_stride, w, h, pitch, layout, color_space, codec,
                                                        blocks, blocks_stride, stream))
+
+    # -- HDR10 P010 (BT.2020, PQ) -> Hap HDR (BC6H): color_space HapB200YUV_BT2020_*, unit_nits the cd/m2 of 1.0 (1-10000),
+    #    texture_format UF16 or SF16; planes as for encode_yuv with HapB200YUV_P010 (pitch default 2 * width); frames need
+    #    max_encoded_length_half(w, h, texture_format, chunks)
+    def encode_yuv_pq(self, luma, chroma, w, h, color_space, unit_nits, texture_format, compressor=1, chunks=1, pitch=None, out=None,
+                      out_capacity=None):
+        """luma, chroma: buffer objects or (addr, nbytes).  Returns (result, frame bytes | used)."""
+        from .abi import _as_ptr
+        laddr, _ = _as_ptr(luma)
+        caddr, _ = _as_ptr(chroma)
+        cap = self.max_encoded_length_half(w, h, texture_format, chunks) if out_capacity is None else out_capacity
+        own = out is None
+        if own:
+            out = bytearray(max(cap, 1))
+        oaddr, _ = _as_ptr(out)
+        used = C.c_ulong(0)
+        r = self.lib.HapB200EncodeYUVPQ(laddr, caddr, w, h, pitch or 2 * w, color_space, unit_nits, texture_format, compressor, chunks,
+                                        oaddr, cap, C.byref(used))
+        if r != 0:
+            return int(r), None
+        return 0, (bytes(memoryview(out)[: used.value]) if own else used.value)
+
+    def encode_yuv_pq_batch(self, luma, chroma, frames, frame_stride, w, h, pitch, color_space, unit_nits, texture_format, compressor,
+                            chunks, out, out_stride, used, stream=None):
+        return int(self.lib.HapB200EncodeYUVPQBatch(luma, chroma, frames, frame_stride, w, h, pitch, color_space, unit_nits,
+                                                    texture_format, compressor, chunks, out, out_stride, used, stream))
+
+    def block_encode_yuv_pq_batch(self, luma, chroma, frames, frame_stride, w, h, pitch, color_space, unit_nits, texture_format, blocks,
+                                  blocks_stride, stream=None):
+        return int(self.lib.HapB200BlockEncodeYUVPQBatch(luma, chroma, frames, frame_stride, w, h, pitch, color_space, unit_nits,
+                                                         texture_format, blocks, blocks_stride, stream))
 
     # -- delivery rings (include/hap_b200.h): frames written straight into another GPU's memory -----------------
     RING_HANDLE_BYTES = 64

@@ -286,11 +286,15 @@ unsigned int HapB200BlockEncodeBC7Batch(const void *rgba, unsigned int frames, u
  *     R = (cy*Yd + crR*Cr8d + 32768) >> 16,  G = (cy*Yd + cbG*Cb8d + crG*Cr8d + 32768) >> 16,  B = (cy*Yd + cbB*Cb8d + 32768) >> 16,
  *   the shift arithmetic, each result clamped to 0..255 (samples outside the nominal range are not clamped first); A = 255. */
 enum HapB200YUVLayout { HapB200YUV_NV12 = 0, HapB200YUV_P010 = 1 };
+/* BT.2020 (non-constant luminance) is taken only by the HDR10 encoders below (HapB200EncodeYUVPQ*); HapB200EncodeYUV*
+ * refuse it: BT.2020 into 8-bit Hap would need tone mapping. */
 enum HapB200YUVColorSpace {
     HapB200YUV_BT601_Limited = 0,
     HapB200YUV_BT601_Full = 1,
     HapB200YUV_BT709_Limited = 2,
-    HapB200YUV_BT709_Full = 3
+    HapB200YUV_BT709_Full = 3,
+    HapB200YUV_BT2020_Limited = 4,
+    HapB200YUV_BT2020_Full = 5
 };
 /* row layout * 4 + colorSpace: {cy, crR, cbG, crG, cbB, yOff, cOff} */
 #define HAPB200_YUV_COEFFICIENTS                                                                                           \
@@ -320,6 +324,59 @@ unsigned int HapB200BlockEncodeYUVBatch(const void *luma, const void *chroma, un
                                         unsigned int width, unsigned int height, unsigned long pitch, unsigned int layout,
                                         unsigned int colorSpace, unsigned int codec, void *blocks, unsigned long blocksStride,
                                         void *stream);
+
+/* ---- Hap HDR (BC6H, "HapH") <- HDR10 P010 (BT.2020, SMPTE ST 2084 / PQ) --------------------------------------------------
+ * The encoders take the P010 pictures a video decoder writes for HEVC Main10 HDR10 and convert them to linear RGBA16F inside
+ * the BC6H encoder, so no RGBA16F picture is ever written.  A P010 picture encodes to exactly the bytes
+ * HapB200EncodeRGBAHalf* give for the RGBA16F picture the conversion below makes of it.
+ * Planes, pitch, geometry and alignment: those of HapB200YUV_P010 for HapB200EncodeYUV* (HDR10 is always 10-bit, so there
+ * is no layout argument).  colorSpace: HapB200YUV_BT2020_Limited or HapB200YUV_BT2020_Full; any other is refused with
+ * HapResult_Bad_Arguments.  textureFormat, compressor, chunkCount, sizes (HapMaxEncodedLength of the one BC6H texture) and
+ * HapResult_Buffer_Too_Small: as for HapB200EncodeRGBAHalf*.  unitNits: the luminance in cd/m2 that the output value 1.0
+ * stands for, an integer from 1 to 10000 (80 for scRGB, 100, or 203 for the BT.2408 HDR reference white are usual); there
+ * is no convention for it shared across tools, so the caller names its working space.  Every argument is checked before
+ * anything touches the GPU.  The first call with a unitNits on a device builds its table (8 KiB) on the host and uploads
+ * it, waiting for the copy; later calls reuse it.
+ * The conversion, exactly:
+ *   1. Chroma upsampling: that of HapB200EncodeYUV, unchanged (Cb8, Cr8 in eighths, default siting, indices clamped).
+ *   2. Matrix to 12-bit R'G'B': the BT.2020 matrix (Kr = 0.2627, Kb = 0.0593), limited range (luma offset 64, luma scale
+ *      876, chroma scale 896) or full range (offset 0, scales 1023), chroma offset 512.  With the row {cy, crR, cbG, crG,
+ *      cbB, yOff, cOff} of HAPB200_YUV_PQ_COEFFICIENTS below (each coefficient round(65536 * 4095 * matrix entry / scale),
+ *      the chroma ones divided by 8 more: the rule of HAPB200_YUV_COEFFICIENTS with 4095 for 255), Yd = Y - yOff,
+ *      Cb8d = Cb8 - 8*cOff and Cr8d = Cr8 - 8*cOff:
+ *        R12 = (cy*Yd + crR*Cr8d + 32768) >> 16,  G12 = (cy*Yd + cbG*Cb8d + crG*Cr8d + 32768) >> 16,
+ *        B12 = (cy*Yd + cbB*Cb8d + 32768) >> 16,
+ *      the shift arithmetic, each clamped to 0..4095 (every intermediate is below 2^30).  12 bits are four times the source's
+ *      resolution, so this rounding adds at most 1/8 of a source code.
+ *   3. Transfer: T[c] is the binary16 of (10000 * EOTF(c / 4095)) / unitNits, rounded once, to nearest, ties to even, where
+ *      EOTF is SMPTE ST 2084's: EOTF(E) = (max(E^(1/m2) - c1, 0) / (c2 - c3 * E^(1/m2)))^(1/m1), m1 = 2610/16384,
+ *      m2 = 2523/32, c1 = 3424/4096, c2 = 2413/128, c3 = 2392/128.  T[0] = 0, T[4095] = the half of 10000 / unitNits;
+ *      every value is finite and non-negative.
+ *   4. The pixel is (T[R12], T[G12], T[B12], 1.0): linear light, in units of unitNits cd/m2, with the BT.2020 primaries
+ *      kept.  Mapping to BT.709 / scRGB primaries (which gives negative values) is left to the caller. */
+/* row colorSpace - HapB200YUV_BT2020_Limited: {cy, crR, cbG, crG, cbB, yOff, cOff} */
+#define HAPB200_YUV_PQ_COEFFICIENTS                                                                                        \
+    {                                                                                                                      \
+        {306358, 55209, -6161, -21391, 70440, 64, 512},  /* P010 BT.2020 limited */                                        \
+        {262336, 48355, -5396, -18736, 61695, 0, 512}    /* P010 BT.2020 full    */                                        \
+    }
+
+/* one P010 picture (host or device pointers) -> one Hap HDR frame */
+unsigned int HapB200EncodeYUVPQ(const void *luma, const void *chroma, unsigned int width, unsigned int height,
+                                unsigned long pitch, unsigned int colorSpace, unsigned int unitNits,
+                                unsigned int textureFormat, unsigned int compressor, unsigned int chunkCount,
+                                void *outputBuffer, unsigned long outputBufferBytes, unsigned long *outputBufferBytesUsed);
+/* frames x P010 picture (device) -> frames x Hap HDR frame at out + f*outStride, encoded length in used[f] (device) */
+unsigned int HapB200EncodeYUVPQBatch(const void *luma, const void *chroma, unsigned int frames, unsigned long frameStride,
+                                     unsigned int width, unsigned int height, unsigned long pitch, unsigned int colorSpace,
+                                     unsigned int unitNits, unsigned int textureFormat, unsigned int compressor,
+                                     unsigned int chunkCount, void *out, unsigned long outStride,
+                                     unsigned long long *used, void *stream);
+/* frames x P010 picture (device) -> bare BC6H textures at blocks + f*blocksStride */
+unsigned int HapB200BlockEncodeYUVPQBatch(const void *luma, const void *chroma, unsigned int frames,
+                                          unsigned long frameStride, unsigned int width, unsigned int height,
+                                          unsigned long pitch, unsigned int colorSpace, unsigned int unitNits,
+                                          unsigned int textureFormat, void *blocks, unsigned long blocksStride, void *stream);
 
 #ifdef __cplusplus
 }

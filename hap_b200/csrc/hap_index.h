@@ -16,7 +16,11 @@
 // lose its place, so the index does not go there).  A frame that carries the index decodes to the same bytes everywhere; a
 // frame without it (every frame the reference writes) is indexed on the fly by snappy_index_kernel.
 // Nothing in the index is trusted: the execute kernel checks that the entries describe exactly the element chain it
-// walks (snappy_decode.cuh), and a chunk whose index does not hold up is decoded again as if it had none.
+// walks (snappy_decode.cuh), and a chunk whose index does not hold up is decoded again as if it had none.  The fragments of
+// an indexed chunk are decoded independently, without waiting for one another, so the index also claims that every copy
+// reads inside its own fragment.  A copy that reaches before its fragment's start is legal Snappy (every other decoder
+// follows it), so such a chunk is not an error: it is decoded again without the index, where windows wait for the windows
+// their copies read.
 //
 // Layout: a section header (4 or 8 bytes, hap.c:137-187) of type kSecFragmentIndex, then the body (little endian, unaligned):
 //   0   'H' 'B' '2' 'I'          magic

@@ -25,7 +25,8 @@
 //       the 16 aligned output bytes of group g from the one to three elements that cover them and writes them with one
 //       128-bit store, so every lane moves the same number of bytes whatever the element lengths are.  Groups whose
 //       source bytes are not final yet wait for a later round; windows of an on-the-fly index wait (one acquire) for
-//       the earlier windows their copies reach into.
+//       the earlier windows their copies reach into.  Fragments of an embedded index made of 8-byte elements (this
+//       encoder's) skip the descriptors and tiles: they are decoded as 4096 eight-byte units (execute_units).
 // Every decision is taken on device; the host reads one status word per chunk.
 #pragma once
 #include "block_primitives.cuh"
@@ -490,13 +491,25 @@ constexpr int kExLook = 16;                          // staged beyond the window
 constexpr int kExTile = HAPB200_EX_TILE;             // output bytes produced per tile
 constexpr int kExGroups = kExTile / 16 + 1;          // a tile that does not start on a 16-byte address touches one group more
 constexpr int kFlattenHops = 12;
+#ifndef HAPB200_EX_UNIT_PATH
+#define HAPB200_EX_UNIT_PATH 1
+#endif
+constexpr uint32_t kExUnits = kIndexFragBytes / 8;   // 8-byte output units of a fragment (unit path)
+constexpr uint32_t kUnitLit = kExUnits;              // unit map value >= this: literal bytes at window byte (value - kUnitLit)
+constexpr int kUnitMaxRounds = 24;                   // pointer jumping over chains of <= 4096 units ends within 13 rounds
+constexpr int kUnitStripLen = 16;                    // units per thread in the unit path's map step
 
 struct ExecSmem {
     uint8_t cin[32 + kExMaxIn + kExLook + 48];       // staged window, cin[32 + a + i] = byte i of the window (32 spare bytes in front)
-    uint32_t e_dst[kExMaxElems];                     // output position inside the chunk
-    uint32_t e_len[kExMaxElems];
-    uint32_t e_a[kExMaxElems];                       // packed source: kSrcIn|input position, kSrcOut|output position, kSrcRun|offset
-    uint32_t e_b[kExMaxElems];                       // destination of the head of the element's same-offset run (its own, if alone)
+    union {
+        struct {
+            uint32_t e_dst[kExMaxElems];             // output position inside the chunk
+            uint32_t e_len[kExMaxElems];
+            uint32_t e_a[kExMaxElems];               // packed source: kSrcIn|input position, kSrcOut|output position, kSrcRun|offset
+            uint32_t e_b[kExMaxElems];               // destination of the head of the element's same-offset run (its own, if alone)
+        };
+        uint16_t umap[2 * kExUnits];                 // unit path: element records, then the source of every 8-byte unit of the fragment
+    };
     uint16_t gfirst[kExGroups + 7];                  // (element + 1) that holds the first byte of an output group
     uint16_t gdone[kExGroups + 7];                   // round in which a group was written (0: not yet)
     uint8_t landed[kExThreads];                      // a chain exit lands in this sub-block
@@ -515,7 +528,7 @@ struct ExecSmem {
         uint32_t min_src;
         int fail;         // walk stage
         int fail_desc;    // descriptor stage
-        int mismatch;     // embedded index does not describe the chain
+        int mismatch;     // embedded index does not describe the chain, or a copy of the fragment reads before it
     } flags[2];
 };
 
@@ -674,6 +687,7 @@ __device__ __forceinline__ bool assemble_group(ExecSmem &S, const TileCtx &C, ui
 struct WalkResult {
     uint32_t exit, count, out_bytes;
     int invalid;
+    uint32_t coarse;   // nonzero: an element's length, or a copy's offset, is not a nonzero multiple of 8
 };
 __device__ __forceinline__ WalkResult walk_piece(const uint8_t *cin, uint32_t wb, uint32_t pos, uint32_t end, uint32_t in_end)
 {
@@ -681,11 +695,14 @@ __device__ __forceinline__ WalkResult walk_piece(const uint8_t *cin, uint32_t wb
     r.count = 0;
     r.out_bytes = 0;
     r.invalid = 0;
+    r.coarse = 0;
     while (pos < end) {
         uint32_t len, aux, hdr, kind;
         if (!read_element_header(cin + pos, wb + pos, in_end, len, aux, hdr, kind)) { r.invalid = 1; break; }
         r.count++;
         r.out_bytes += len;
+        r.coarse |= (len | (kind == 0 ? 0u : aux)) & 7u;
+        if (kind != 0 && aux == 0) r.coarse = 1;
         pos += hdr + (kind == 0 ? len : 0);
     }
     r.exit = pos;
@@ -707,6 +724,131 @@ __device__ __noinline__ void fetch_next_window(const ChunkJob *jobs, uint32_t nj
     }
     *ticket_out = w;
     if (w != 0xFFFFFFFFu) *win_out = wins[w];
+}
+
+#ifdef HAPB200_EMU
+inline uint64_t &emu_unit_windows() { static uint64_t n = 0; return n; }   // windows the unit path decoded (tests only)
+#endif
+
+// The unit path: a fragment of an embedded index whose elements are all 8-byte granular (every length and copy offset a
+// nonzero multiple of 8: what this repo's encoder writes) is 4096 units of 8 bytes, each either 8 literal bytes of the
+// staged stream or a copy of an earlier unit.  No descriptors, passes, runs or output-centric rounds are needed:
+//   records: every piece's walk writes one 16-bit record at the first unit of each element (kUnitLit + stream position of a
+//            literal, the distance in units of a copy; 0 = no element starts at this unit);
+//   map:     thread t owns units 16t .. 16t + 15; a max-scan finds the element each unit lies in, and the unit gets
+//            kUnitLit + its stream position (literal) or the earlier unit it copies (the element's period for overlapping
+//            copies): every lane does the same work whatever the element lengths are;
+//   resolve: map[u] = map[map[u]] in rounds until every unit names stream bytes (sources are strictly earlier units of the
+//            fragment, so every chain ends at a literal; a racing update only skips hops);
+//   write:   thread g assembles destination-aligned 16-byte group g from two or three units of the staged window.
+// Called by all threads behind the walk checks (total_o == out_len <= 32 KiB).  Returns false (uniform) when a copy reads
+// before the fragment or before the chunk: the caller hands the chunk to the repair pass.  `coff`: cin byte of window byte 0;
+// `crossing`: the window's flag that is not tested behind the walk's barrier (set here by the thread that finds such a copy).
+__device__ __noinline__ bool execute_units(ExecSmem &S, int &crossing, uint32_t coff, uint32_t wb, uint32_t in_end, bool entered,
+                                           uint32_t pos, uint32_t end, uint32_t obase, uint8_t *out, uint32_t out_len)
+{
+    static_assert(kExUnits == kUnitStripLen * kExThreads, "16 units per thread");
+    const int t = threadIdx.x;
+    uint16_t *rec = S.umap, *map = S.umap + kExUnits;
+    const uint8_t *cin = S.cin + coff;
+    uint4 *rec4 = reinterpret_cast<uint4 *>(rec), *map4 = reinterpret_cast<uint4 *>(map);
+    rec4[2 * t] = make_uint4(0, 0, 0, 0);
+    rec4[2 * t + 1] = make_uint4(0, 0, 0, 0);
+    __syncthreads();
+    if (entered) {
+        uint32_t u = obase >> 3;   // (a multiple of 8: every element before this piece is)
+        while (pos < end) {
+            uint32_t len, aux, hdr, kind;
+            read_element_header(cin + pos, wb + pos, in_end, len, aux, hdr, kind);   // (the walk checked every header)
+            if (kind == 0) {
+                rec[u] = (uint16_t)(kUnitLit + (aux - wb));
+                pos += hdr + len;
+            } else {
+                const uint32_t d = aux >> 3;
+                if (d > u) { crossing = 1; break; }
+                rec[u] = (uint16_t)d;
+                pos += hdr;
+            }
+            u += len >> 3;
+        }
+    }
+    __syncthreads();
+    if (crossing) return false;
+    const uint32_t U = out_len >> 3, u0 = kUnitStripLen * (uint32_t)t;
+    uint32_t r[kUnitStripLen];
+    {
+        const uint4 a = rec4[2 * t], b = rec4[2 * t + 1];
+        const uint32_t w[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+#pragma unroll
+        for (int k = 0; k < kUnitStripLen; k++) r[k] = (w[k >> 1] >> (16 * (k & 1))) & 0xFFFFu;
+    }
+    uint32_t last = 0;   // (unit + 1) of the last element start in this strip
+#pragma unroll
+    for (int k = 0; k < kUnitStripLen; k++) last = r[k] != 0 ? u0 + k + 1 : last;
+    uint32_t unused;
+    const uint32_t carry = block_excl_max<kExThreads>(last, &unused, S.scratch);   // the element running into this strip
+    uint32_t start = carry ? carry - 1 : 0, rs = carry ? rec[carry - 1] : 0;
+    int pending = 0;   // a unit still names another unit
+    uint32_t v[kUnitStripLen];
+#pragma unroll
+    for (int k = 0; k < kUnitStripLen; k++) {
+        const uint32_t u = u0 + k;
+        if (r[k] != 0) { start = u; rs = r[k]; }
+        const uint32_t q = u - start;
+        v[k] = rs >= kUnitLit ? rs + 8 * q : start - rs + (q < rs || rs == 0 ? q : q % rs);   // (rs == 0: only past unit U)
+        pending |= u < U && v[k] < kUnitLit;
+    }
+#pragma unroll
+    for (int h = 0; h < 2; h++)
+        map4[2 * t + h] = make_uint4((v[8 * h] & 0xFFFFu) | (v[8 * h + 1] << 16), (v[8 * h + 2] & 0xFFFFu) | (v[8 * h + 3] << 16),
+                                     (v[8 * h + 4] & 0xFFFFu) | (v[8 * h + 5] << 16), (v[8 * h + 6] & 0xFFFFu) | (v[8 * h + 7] << 16));
+    pending = __syncthreads_or(pending);
+    for (int round = 0; pending; round++) {
+        pending = 0;
+        for (uint32_t u = t; u < U; u += kExThreads) {
+            const uint32_t v = map[u];
+            if (v < kUnitLit) {
+                const uint32_t v2 = map[v];
+                map[u] = (uint16_t)v2;
+                pending |= v2 < kUnitLit;
+            }
+        }
+        pending = __syncthreads_or(pending);
+        if (pending && round == kUnitMaxRounds) return false;   // (cannot happen: chains are at most 4096 units deep)
+    }
+    // group g = destination bytes [16g - m, 16g - m + 16) of the fragment, m = misalignment of its first byte
+    const uint32_t *c32 = reinterpret_cast<const uint32_t *>(S.cin);
+    const uint32_t m = (uint32_t)((uintptr_t)out & 15);
+    const uint32_t ngroups = (m + out_len + 15) >> 4;
+    for (uint32_t g = t; g < ngroups; g += kExThreads) {
+        const int32_t x = 16 * (int32_t)g - (int32_t)m;
+        const int32_t ua = x >> 3;   // (floor: -2 or -1 for the first group of a misaligned fragment)
+        const uint32_t r = (uint32_t)x & 7u;
+        uint32_t w[6];
+#pragma unroll
+        for (int k = 0; k < 3; k++) {
+            const int32_t u = ua + k;
+            w[2 * k] = 0;
+            w[2 * k + 1] = 0;
+            if (u >= 0 && (uint32_t)u < U && (k < 2 || r != 0)) {
+                const uint32_t b = coff + (uint32_t)map[u] - kUnitLit, i = b >> 2, sh = 8 * (b & 3);
+                const uint32_t s0 = c32[i], s1 = c32[i + 1], s2 = c32[i + 2];
+                w[2 * k] = __funnelshift_r(s0, s1, sh);
+                w[2 * k + 1] = __funnelshift_r(s1, s2, sh);
+            }
+        }
+        const uint32_t q = r >> 2, sh = 8 * (r & 3);
+        const uint32_t o0 = __funnelshift_r(w[q], w[q + 1], sh), o1 = __funnelshift_r(w[q + 1], w[q + 2], sh);
+        const uint32_t o2 = __funnelshift_r(w[q + 2], w[q + 3], sh), o3 = __funnelshift_r(w[q + 3], w[q + 4], sh);
+        if (x >= 0 && (uint32_t)x + 16 <= out_len) {
+            *reinterpret_cast<uint4 *>(out + x) = make_uint4(o0, o1, o2, o3);   // 16-byte aligned by the choice of m
+        } else {
+            const uint32_t ow[4] = {o0, o1, o2, o3};
+            for (int i = 0; i < 16; i++)
+                if (x + i >= 0 && (uint32_t)(x + i) < out_len) out[x + i] = (uint8_t)(ow[i >> 2] >> (8 * (i & 3)));
+        }
+    }
+    return true;
 }
 
 // pass 0 executes the chunks in mode kJobReady, pass 1 (repair) those in mode kJobRepaired.
@@ -787,7 +929,7 @@ __global__ void __launch_bounds__(kExThreads, HAPB200_EX_MIN_BLOCKS) snappy_exec
         const uint32_t my_hi = ((uint32_t)t + 1 == nsub) ? win.in_len : ((uint32_t)t + 1) * sub;
         const bool entered = (uint32_t)t < nsub && ent != kIndexNoEntry;
         WalkResult wr;
-        wr.exit = 0; wr.count = 0; wr.out_bytes = 0; wr.invalid = 0;
+        wr.exit = 0; wr.count = 0; wr.out_bytes = 0; wr.invalid = 0; wr.coarse = 0;
         if (entered) {
             if (my_lo + ent >= my_hi) {
                 wr.invalid = 1;
@@ -820,11 +962,33 @@ __global__ void __launch_bounds__(kExThreads, HAPB200_EX_MIN_BLOCKS) snappy_exec
             }
         }
         if (t == 0 && total_o != win.out_len) F.fail = 1;
+#if HAPB200_EX_UNIT_PATH
+        const bool coarse = __syncthreads_or(wr.coarse != 0) != 0;   // the barrier the checks below need, OR-ing the walk's grain test
+#else
         __syncthreads();
+#endif
         if (F.fail || F.mismatch) {
             if (t == 0) { job.status = embedded ? kStatusIndexMismatch : (uint32_t)HapResult_Bad_Frame; __threadfence(); hap_st_release(&done[w], 1u); }
             continue;
         }
+#if HAPB200_EX_UNIT_PATH
+        if (embedded && !coarse) {
+            // A copy that reads before the fragment is flagged in fail_desc, the descriptor stage's flag: mismatch may still be
+            // tested by slower threads behind the barrier above.  Either way the chunk ends as kStatusIndexMismatch (repair).
+            int &crossing = F.fail_desc;
+            const bool ok = execute_units(S, crossing, 32 + a_sh, wb, in_end, entered, my_lo + ent, my_hi, obase, dst + win.out_off, win.out_len);
+            __syncthreads();
+            if (t == 0) {
+                if (!ok) job.status = kStatusIndexMismatch;
+#ifdef HAPB200_EMU
+                else emu_unit_windows()++;
+#endif
+                __threadfence();
+                hap_st_release(&done[w], 1u);
+            }
+            continue;
+        }
+#endif
 
         // ---- passes: as many pieces as the descriptor arrays hold -------------------------------------------------------------
         uint32_t pbase_e = 0;
@@ -877,6 +1041,10 @@ __global__ void __launch_bounds__(kExThreads, HAPB200_EX_MIN_BLOCKS) snappy_exec
                     e++;
                 }
                 if (!waited && msrc < win.out_off) atomicMin(&F.min_src, msrc);
+                // a fragment of an embedded index is decoded without waiting for the others: a copy that reads before it
+                // is legal Snappy, but only the repair pass (on-the-fly index, with waits) may execute it
+                // (fail_desc, not mismatch: slower threads may still be testing mismatch behind the walk's barrier)
+                if (embedded && msrc < win.out_off) F.fail_desc = 1;
             }
             __syncthreads();
             if (F.fail_desc) { bad = true; break; }

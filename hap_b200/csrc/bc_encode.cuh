@@ -51,6 +51,25 @@ HAP_HD BcGeom bc_encode_geom(uint32_t width, uint32_t height, uint32_t row_bytes
 // CTAs per frame of the block kernels (encode and decode): one thread per block
 HAP_HD uint32_t bc_ctas(uint32_t blocks_x, uint32_t blocks_y) { return (uint32_t)(((uint64_t)blocks_x * blocks_y + kBcThreads - 1) / kBcThreads); }
 
+// Column and row of block bi (row-major) without a division: the multiply-high estimate of the row is exact or one short.
+__device__ __forceinline__ void block_xy(uint32_t bi, uint32_t blocks_x, uint32_t inv_blocks_x, uint32_t &bx, uint32_t &by)
+{
+    by = __umulhi(bi, inv_blocks_x);
+    bx = bi - by * blocks_x;
+    if (bx >= blocks_x) { by++; bx -= blocks_x; }
+}
+
+// The 16 texels of block (bx, by) of the RGBA8 picture at `pic`: one 16-byte load per pixel row.
+__device__ __forceinline__ void load_block_rgba8(const uint8_t *pic, uint32_t row_bytes, uint32_t bx, uint32_t by, uint32_t px[16])
+{
+    const uint8_t *src = pic + (uint64_t)(4 * by) * row_bytes + 16u * bx;
+#pragma unroll
+    for (int row = 0; row < 4; row++) {
+        uint4 v = *reinterpret_cast<const uint4 *>(src + (uint64_t)row * row_bytes);
+        px[4 * row + 0] = v.x; px[4 * row + 1] = v.y; px[4 * row + 2] = v.z; px[4 * row + 3] = v.w;
+    }
+}
+
 // The frame is blockIdx.y, and gridDim.y is at most 65535: batches of more frames are launched in slices of this many.
 constexpr uint32_t kBcFramesPerLaunch = 65535;
 
@@ -66,16 +85,11 @@ __global__ void __launch_bounds__(kBcThreads, (KIND == kBcYCoCg && !REFINE) ? 7 
     const uint32_t nblocks = G.blocks_x * G.blocks_y;
     const uint32_t bi = blockIdx.x * kBcThreads + threadIdx.x;
     if (bi >= nblocks) return;
-    uint32_t by = __umulhi(bi, G.inv_blocks_x), bx = bi - by * G.blocks_x;  // the estimate is exact or one short
-    if (bx >= G.blocks_x) { by++; bx -= G.blocks_x; }
+    uint32_t bx, by;
+    block_xy(bi, G.blocks_x, G.inv_blocks_x, bx, by);
     uint32_t px[16];
     if (SRC == kSrcRgba8) {
-        const uint8_t *src = rgba + (uint64_t)blockIdx.y * G.frame_bytes + (uint64_t)(4 * by) * G.row_bytes + 16u * bx;
-#pragma unroll
-        for (int row = 0; row < 4; row++) {
-            uint4 v = *reinterpret_cast<const uint4 *>(src + (uint64_t)row * G.row_bytes);
-            px[4 * row + 0] = v.x; px[4 * row + 1] = v.y; px[4 * row + 2] = v.z; px[4 * row + 3] = v.w;
-        }
+        load_block_rgba8(rgba + (uint64_t)blockIdx.y * G.frame_bytes, G.row_bytes, bx, by, px);
     } else {
         const uint64_t f = (uint64_t)blockIdx.y * G.frame_bytes;
         load_block_yuv<SRC>(rgba + f, Y.chroma + f, G.row_bytes, bx, by, G.blocks_x, G.blocks_y, Y, px);

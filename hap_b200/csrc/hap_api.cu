@@ -14,6 +14,7 @@
 #include "hap_host.h"
 #include "hap_mov.h"
 #include "hap_parse.cuh"
+#include "hapq_fused.cuh"
 #include "snappy_decode.cuh"
 #include "snappy_encode.cuh"
 
@@ -89,6 +90,7 @@ struct DeviceState {
     bool ready = false;
     int sm_count = 132;
     int k5_ctas_per_sm = 1;   // resident CTAs of the fragment compressor per SM (its persistent grid is this x sm_count)
+    int fused_ctas_per_sm = 1;   // the same for the fused Hap Q encoder (hapq_fused.cuh)
 };
 DeviceState g_dev[kMaxDevices];
 std::atomic<int> g_default_device{-1};
@@ -111,8 +113,12 @@ void device_init(int dev)
                                     (int)sizeof(EncodeSmem)) == cudaSuccess;
     ok = ok && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&d.k5_ctas_per_sm, snappy_encode_fragments_kernel, kEncThreads,
                                                              sizeof(EncodeSmem)) == cudaSuccess;
+    ok = ok && cudaFuncSetAttribute(hapq_fused_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(EncodeSmem)) == cudaSuccess;
+    ok = ok && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&d.fused_ctas_per_sm, hapq_fused_encode_kernel, kEncThreads,
+                                                             sizeof(EncodeSmem)) == cudaSuccess;
     if (!ok) { cudaGetLastError(); return; }
     if (d.k5_ctas_per_sm < 1) d.k5_ctas_per_sm = 1;
+    if (d.fused_ctas_per_sm < 1) d.fused_ctas_per_sm = 1;
     d.ready = true;
 }
 
@@ -310,10 +316,18 @@ uint32_t on_batch_stream(void *stream, Work &&work)
 
 // ---- device pipelines (all asynchronous on `st`) -------------------------------------------------
 
+// The RGBA8 pictures the fused Hap Q encoder fits its blocks from (geometry g: g.frame_bytes apart, rows g.row_bytes apart).
+struct FusedPictures {
+    const uint8_t *rgba;
+    BcGeom g;
+};
+
 // textures of `frames` frames (device, described by G.s[i].in_offset/in_stride relative to `base`) ->
-// frames at out + f*out_stride, lengths in used[f]
+// frames at out + f*out_stride, lengths in used[f].
+// fused: the textures are not there yet; the fused Hap Q encoder fits them from these pictures, writes them to `base` and
+// compresses them in one kernel, in place of the fragment compressor (G must pass fused_hapq_geometry).
 uint32_t launch_encode(const uint8_t *base, const FrameGeom &G, uint32_t frames, uint8_t *out, uint64_t out_stride,
-                       unsigned long long *used, cudaStream_t st)
+                       unsigned long long *used, cudaStream_t st, const FusedPictures *fused = nullptr)
 {
     const uint64_t nfrag = (uint64_t)frames * G.frags_per_frame;
     if (nfrag == 0 || nfrag >= (1ull << 31)) return HapResult_Bad_Arguments;
@@ -327,10 +341,15 @@ uint32_t launch_encode(const uint8_t *base, const FrameGeom &G, uint32_t frames,
         return HapResult_Internal_Error;
     }
     // every CTA that can be resident at once (two per SM with the kernel's 108 KB of shared memory) strides over the fragments
-    const uint64_t k5_resident = (uint64_t)sm_count() * (uint64_t)g_dev[t_device].k5_ctas_per_sm;
+    const uint64_t k5_resident = (uint64_t)sm_count() * (uint64_t)(fused ? g_dev[t_device].fused_ctas_per_sm : g_dev[t_device].k5_ctas_per_sm);
     const unsigned k5_grid = (unsigned)(nfrag < k5_resident ? nfrag : k5_resident);
-    HAP_KLAUNCH(kStSnappyEncode, snappy_encode_fragments_kernel, dim3(k5_grid), dim3(kEncThreads), sizeof(EncodeSmem), st, base, G,
-                (uint32_t)nfrag, scratch.as<uint8_t>(), fsize.as<uint32_t>(), write_index ? fent.as<uint8_t>() : (uint8_t *)nullptr);
+    uint8_t *entries = write_index ? fent.as<uint8_t>() : (uint8_t *)nullptr;
+    if (fused)   // (counted as block encoding: the fit is most of its work)
+        HAP_KLAUNCH(kStBcEncode, hapq_fused_encode_kernel, dim3(k5_grid), dim3(kEncThreads), sizeof(EncodeSmem), st, fused->rgba, fused->g,
+                    const_cast<uint8_t *>(base), G, (uint32_t)nfrag, scratch.as<uint8_t>(), fsize.as<uint32_t>(), entries);
+    else
+        HAP_KLAUNCH(kStSnappyEncode, snappy_encode_fragments_kernel, dim3(k5_grid), dim3(kEncThreads), sizeof(EncodeSmem), st, base, G,
+                    (uint32_t)nfrag, scratch.as<uint8_t>(), fsize.as<uint32_t>(), entries);
     HAP_KLAUNCH(kStPlan, hap_plan_frames_kernel, dim3(frames), dim3(kPlanThreads), 0, st, G, base, fsize.as<uint32_t>(),
                 fdst.as<uint32_t>(), fidx.as<uint32_t>(), (write_index ? kPlanWriteIndex : 0u) | (g_write_offsets.load() ? kPlanWriteOffsets : 0u), out,
                 out_stride, used);
@@ -469,26 +488,30 @@ uint32_t launch_bc6h_encode(const PictureSrc &p, uint32_t frames, uint64_t frame
 
 // The tail of the picture batch encoders: encode_blocks(textures, stride) fills the textures of every frame into device
 // scratch (frame f at textures + f*stride, texture 1 at align16(t[0]) inside it), then the frames are laid out from them at
-// out + f*out_stride, lengths in used[f].
+// out + f*out_stride, lengths in used[f].  fused: Hap Q pictures the fused encoder may take (hapq_fused.cuh); it does when the
+// texture's chunks pass fused_hapq_geometry, and encode_blocks is not called then.
 template <class EncodeBlocks>
 uint32_t encode_frames_from_blocks(uint32_t frames, uint32_t count, const uint64_t t[2], const uint32_t fmt[2], unsigned compressor,
                                    unsigned chunk_count, uint8_t *out, uint64_t out_stride, unsigned long long *used, cudaStream_t st,
-                                   EncodeBlocks &&encode_blocks)
+                                   EncodeBlocks &&encode_blocks, const FusedPictures *fused = nullptr)
 {
     const uint64_t stride = align16(t[0]) + align16(t[1]);
     DevBuf tex(st);
     if (!tex.alloc(stride * frames + 16)) { cudaGetLastError(); return (uint32_t)HapResult_Internal_Error; }
-    uint32_t r = encode_blocks(tex.as<uint8_t>(), stride);
-    if (r != HapResult_No_Error) return r;
     TextureArgs ta[2] = {{t[0], fmt[0], compressor, chunk_count}, {t[1], fmt[1], compressor, chunk_count}};
     FrameGeom G;
-    r = build_frame_geom(count, ta, G);
+    uint32_t r = build_frame_geom(count, ta, G);
     if (r != HapResult_No_Error) return r;
     for (unsigned i = 0; i < count; i++) {
         G.s[i].in_offset = i ? align16(t[0]) : 0;
         G.s[i].in_stride = stride;
     }
-    return launch_encode(tex.as<uint8_t>(), G, frames, out, out_stride, used, st);
+    if (fused && !fused_hapq_geometry(G)) fused = nullptr;
+    if (!fused) {
+        r = encode_blocks(tex.as<uint8_t>(), stride);
+        if (r != HapResult_No_Error) return r;
+    }
+    return launch_encode(tex.as<uint8_t>(), G, frames, out, out_stride, used, st, fused);
 }
 
 template <int KIND>
@@ -1242,13 +1265,19 @@ static unsigned encode_picture_batch(const CodecInfo &ci, const PictureSrc &p, u
         return HapResult_Bad_Arguments;
     if (outStride < max_encoded_length_rgba(width, height, ci, chunkCount)) return HapResult_Buffer_Too_Small;
     HAP_ENTER(p.pixels, out);
+    // Hap Q from RGBA8 without the chroma refinement, Snappy: the fused encoder (hapq_fused.cuh) when the chunks allow it
+    const FusedPictures fp = {(const uint8_t *)p.pixels, bc_encode_geom(width, height, (uint32_t)pitch, frameStride, 0, 0)};
+    const bool fuse = HAPB200_FUSED_HAPQ && ci.bc_kind == kBcYCoCg && p.kind == kSrcRgba8 && g_chroma_refine.load() == 0 &&
+                      compressor == HapCompressorSnappy;
     return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
         const uint64_t t[2] = {texture_bytes(width, height, ci, 0), texture_bytes(width, height, ci, 1)};
-        return encode_frames_from_blocks(frames, ci.textures, t, ci.fmt, compressor, chunkCount, (uint8_t *)out, outStride, used, st,
-                                         [&](uint8_t *tex, uint64_t stride) {
-                                             return launch_block_encode((const uint8_t *)p.pixels, frames, frameStride, width, height, pitch, ci,
-                                                                        tex, stride, align16(t[0]), st, p.kind, p.yuv());
-                                         });
+        return encode_frames_from_blocks(
+            frames, ci.textures, t, ci.fmt, compressor, chunkCount, (uint8_t *)out, outStride, used, st,
+            [&](uint8_t *tex, uint64_t stride) {
+                return launch_block_encode((const uint8_t *)p.pixels, frames, frameStride, width, height, pitch, ci, tex, stride, align16(t[0]),
+                                           st, p.kind, p.yuv());
+            },
+            fuse ? &fp : nullptr);
     });
 }
 

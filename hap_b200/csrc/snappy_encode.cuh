@@ -336,6 +336,8 @@ struct FragRef {
     const uint8_t *in;
     bool second;         // fragment of the frame's second texture
     uint32_t units;      // 8-byte units; 0: the section is not compressed (fragment stored raw)
+    uint32_t frame;      // frame of the batch
+    uint32_t tex_off;    // byte offset of the fragment inside its texture
 };
 // x / d and x % d with a multiplication: magic = floor(2^32 / d) (0xFFFFFFFF for d = 1), one correction step
 __device__ __forceinline__ uint32_t fast_divmod(uint32_t x, uint32_t d, uint32_t magic, uint32_t &rem)
@@ -368,6 +370,8 @@ __device__ __forceinline__ FragRef locate_fragment(const uint8_t *dxt, const Fra
     const uint32_t left = chunk_bytes - j * kFragBytes;
     r.units = compress ? (left < (uint32_t)kFragBytes ? left : (uint32_t)kFragBytes) >> 3 : 0u;
     r.second = second;
+    r.frame = frame;
+    r.tex_off = chunk * chunk_bytes + j * (uint32_t)kFragBytes;   // (a section is under 2 GiB: build_frame_geom)
     return r;
 }
 
@@ -396,6 +400,31 @@ __device__ __forceinline__ void load_strip(const FragRef &fr, uint32_t i0, uint2
     }
 }
 
+// Copies fragment gfrag's element stream (`total` bytes in S.out) and index entries out of shared memory, records its size,
+// and waits until every thread is done with the fragment's shared memory.
+__device__ __forceinline__ void store_fragment(const EncodeSmem &S, uint32_t total, uint32_t gfrag, uint8_t *__restrict__ scratch,
+                                               uint32_t *__restrict__ frag_size, uint8_t *__restrict__ frag_entries)
+{
+    const uint32_t t = threadIdx.x;
+    uint8_t *o = scratch + (uint64_t)gfrag * kFragCap;
+    const uint4 *o4s = reinterpret_cast<const uint4 *>(S.out);
+    uint4 *o4 = reinterpret_cast<uint4 *>(o);       // (scratch slots are kFragCap = 32800 bytes apart: 16-byte aligned)
+    for (uint32_t i = t; i < (total + 15) / 16; i += kEncThreads) o4[i] = o4s[i];
+    if (frag_entries != nullptr && t < kFragEntryStride) frag_entries[(uint64_t)gfrag * kFragEntryStride + t] = (uint8_t)S.entry[t];
+    if (t == 0) frag_size[gfrag] = total;
+    __syncthreads();   // S.out, S.data and the tables are rewritten by the next fragment
+}
+
+// The table and the index entries of a fragment start empty (before the barrier in front of compress_fragment).
+__device__ __forceinline__ void init_fragment_tables(EncodeSmem &S)
+{
+    const int t = threadIdx.x;
+    uint4 *tb = reinterpret_cast<uint4 *>(S.u.table);
+    const uint4 ones = make_uint4(0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu);
+    for (int q = t; q < (1 << kEncHashBits) / 4; q += kEncThreads) tb[q] = ones;
+    if (t < kFragEntryStride) S.entry[t] = kIndexNoEntry;
+}
+
 // A persistent grid (as many CTAs as fit on the device at once: two per SM, the kernel needs 108 KB of shared memory)
 // strides over the nfrag = frames * frags_per_frame fragments of the batch.  While one CTA of an SM waits at a barrier
 // or for the HBM latency of its next fragment's input, the other one computes.
@@ -420,23 +449,12 @@ __global__ void __launch_bounds__(kEncThreads, 2) snappy_encode_fragments_kernel
         load_strip(cur, i0, d);
 #pragma unroll
         for (int k = 0; k < kUnitStrip; k += 2) *reinterpret_cast<uint4 *>(&S.data[i0 + k]) = make_uint4(d[k].x, d[k].y, d[k + 1].x, d[k + 1].y);
-        {
-            uint4 *tb = reinterpret_cast<uint4 *>(S.u.table);
-            const uint4 ones = make_uint4(0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu);
-            for (int q = t; q < (1 << kEncHashBits) / 4; q += kEncThreads) tb[q] = ones;
-            if (t < kFragEntryStride) S.entry[t] = kIndexNoEntry;
-        }
+        init_fragment_tables(S);
         __syncthreads();
         const uint32_t period_units = (cur.second ? G.s[1].period_words : G.s[0].period_words) >> 1;   // 8-byte blocks: 1, 16-byte blocks: 2
         const uint32_t total = U == (uint32_t)kFragUnits ? compress_fragment<true>(S, d, U, period_units)
                                                          : compress_fragment<false>(S, d, U, period_units);
-        uint8_t *o = scratch + (uint64_t)gfrag * kFragCap;
-        const uint4 *o4s = reinterpret_cast<const uint4 *>(S.out);
-        uint4 *o4 = reinterpret_cast<uint4 *>(o);       // (scratch slots are kFragCap = 32800 bytes apart: 16-byte aligned)
-        for (uint32_t i = t; i < (total + 15) / 16; i += kEncThreads) o4[i] = o4s[i];
-        if (frag_entries != nullptr && t < kFragEntryStride) frag_entries[(uint64_t)gfrag * kFragEntryStride + t] = (uint8_t)S.entry[t];
-        if (t == 0) frag_size[gfrag] = total;
-        __syncthreads();   // S.out, S.data and the tables are rewritten by the next fragment
+        store_fragment(S, total, gfrag, scratch, frag_size, frag_entries);
     }
 }
 

@@ -91,6 +91,7 @@ struct DeviceState {
     int sm_count = 132;
     int k5_ctas_per_sm = 1;   // resident CTAs of the fragment compressor per SM (its persistent grid is this x sm_count)
     int fused_ctas_per_sm = 1;   // the same for the fused Hap Q encoder (hapq_fused.cuh)
+    int fused_place_ctas_per_sm = 1;   // ... and for its variant that writes the frames itself
 };
 DeviceState g_dev[kMaxDevices];
 std::atomic<int> g_default_device{-1};
@@ -116,7 +117,11 @@ void device_init(int dev)
     ok = ok && cudaFuncSetAttribute(hapq_fused_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(EncodeSmem)) == cudaSuccess;
     ok = ok && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&d.fused_ctas_per_sm, hapq_fused_encode_kernel, kEncThreads,
                                                              sizeof(EncodeSmem)) == cudaSuccess;
+    ok = ok && cudaFuncSetAttribute(hapq_fused_place_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(EncodeSmem)) == cudaSuccess;
+    ok = ok && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&d.fused_place_ctas_per_sm, hapq_fused_place_kernel, kEncThreads,
+                                                             sizeof(EncodeSmem)) == cudaSuccess;
     if (!ok) { cudaGetLastError(); return; }
+    if (d.fused_place_ctas_per_sm < 1) d.fused_place_ctas_per_sm = 1;
     if (d.k5_ctas_per_sm < 1) d.k5_ctas_per_sm = 1;
     if (d.fused_ctas_per_sm < 1) d.fused_ctas_per_sm = 1;
     d.ready = true;
@@ -325,7 +330,8 @@ struct FusedPictures {
 // textures of `frames` frames (device, described by G.s[i].in_offset/in_stride relative to `base`) ->
 // frames at out + f*out_stride, lengths in used[f].
 // fused: the textures are not there yet; the fused Hap Q encoder fits them from these pictures, writes them to `base` and
-// compresses them in one kernel, in place of the fragment compressor (G must pass fused_hapq_geometry).
+// compresses them in one kernel, in place of the fragment compressor (G must pass fused_hapq_geometry).  Without the offset
+// table it also writes the streams into the frames (hapq_fused_place_kernel), and the place kernel copies raw fragments only.
 uint32_t launch_encode(const uint8_t *base, const FrameGeom &G, uint32_t frames, uint8_t *out, uint64_t out_stride,
                        unsigned long long *used, cudaStream_t st, const FusedPictures *fused = nullptr)
 {
@@ -340,10 +346,35 @@ uint32_t launch_encode(const uint8_t *base, const FrameGeom &G, uint32_t frames,
         cudaGetLastError();
         return HapResult_Internal_Error;
     }
+    const bool write_offsets = g_write_offsets.load();
+    const uint32_t plan_flags = (write_index ? kPlanWriteIndex : 0u) | (write_offsets ? kPlanWriteOffsets : 0u);
+    uint8_t *entries = write_index ? fent.as<uint8_t>() : (uint8_t *)nullptr;
+    if (HAPB200_FUSED_PLACE && fused && !write_offsets) {
+        // The fused encoder writes the element streams into the frames itself; the plan kernel lists the raw fragments
+        // for the place kernel.  sync = ticket, raw-fragment count, published sizes [nfrag], next-chunk starts [nfrag].
+        DevBuf sync(st), work(st);
+        const size_t sync_bytes = (2 + 2 * nfrag) * 4;
+        if (!sync.alloc(sync_bytes) || !work.alloc(nfrag * 4) || cudaMemsetAsync(sync.p, 0, sync_bytes, st) != cudaSuccess) {
+            cudaGetLastError();
+            return HapResult_Internal_Error;
+        }
+        uint32_t *sy = sync.as<uint32_t>();
+        const FusedPlaceArgs P{out, out_stride, sy, sy + 2, sy + 2 + nfrag};
+        const uint64_t resident = (uint64_t)sm_count() * (uint64_t)g_dev[t_device].fused_place_ctas_per_sm;
+        HAP_KLAUNCH(kStBcEncode, hapq_fused_place_kernel, dim3((unsigned)(nfrag < resident ? nfrag : resident)), dim3(kEncThreads),
+                    sizeof(EncodeSmem), st, fused->rgba, fused->g, const_cast<uint8_t *>(base), G, (uint32_t)nfrag, scratch.as<uint8_t>(),
+                    fsize.as<uint32_t>(), entries, P);
+        HAP_KLAUNCH(kStPlan, hap_plan_placed_frames_kernel, dim3(frames), dim3(kPlanThreads), 0, st, G, base, fsize.as<uint32_t>(),
+                    fdst.as<uint32_t>(), fidx.as<uint32_t>(), plan_flags, out, out_stride, used,
+                    PlanPlaced{scratch.as<uint8_t>(), entries, work.as<uint32_t>(), sy + 1});
+        const uint64_t place_grid = (uint64_t)sm_count() * 8;   // 8 CTAs of 256 threads fill an SM
+        HAP_KLAUNCH(kStPlace, hap_place_listed_kernel, dim3((unsigned)(nfrag < place_grid ? nfrag : place_grid)), dim3(kPlaceThreads), 0, st,
+                    G, base, fsize.as<uint32_t>(), fdst.as<uint32_t>(), work.as<uint32_t>(), sy + 1, out, out_stride);
+        return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
+    }
     // every CTA that can be resident at once (two per SM with the kernel's 108 KB of shared memory) strides over the fragments
     const uint64_t k5_resident = (uint64_t)sm_count() * (uint64_t)(fused ? g_dev[t_device].fused_ctas_per_sm : g_dev[t_device].k5_ctas_per_sm);
     const unsigned k5_grid = (unsigned)(nfrag < k5_resident ? nfrag : k5_resident);
-    uint8_t *entries = write_index ? fent.as<uint8_t>() : (uint8_t *)nullptr;
     if (fused)   // (counted as block encoding: the fit is most of its work)
         HAP_KLAUNCH(kStBcEncode, hapq_fused_encode_kernel, dim3(k5_grid), dim3(kEncThreads), sizeof(EncodeSmem), st, fused->rgba, fused->g,
                     const_cast<uint8_t *>(base), G, (uint32_t)nfrag, scratch.as<uint8_t>(), fsize.as<uint32_t>(), entries);
@@ -351,8 +382,7 @@ uint32_t launch_encode(const uint8_t *base, const FrameGeom &G, uint32_t frames,
         HAP_KLAUNCH(kStSnappyEncode, snappy_encode_fragments_kernel, dim3(k5_grid), dim3(kEncThreads), sizeof(EncodeSmem), st, base, G,
                     (uint32_t)nfrag, scratch.as<uint8_t>(), fsize.as<uint32_t>(), entries);
     HAP_KLAUNCH(kStPlan, hap_plan_frames_kernel, dim3(frames), dim3(kPlanThreads), 0, st, G, base, fsize.as<uint32_t>(),
-                fdst.as<uint32_t>(), fidx.as<uint32_t>(), (write_index ? kPlanWriteIndex : 0u) | (g_write_offsets.load() ? kPlanWriteOffsets : 0u), out,
-                out_stride, used);
+                fdst.as<uint32_t>(), fidx.as<uint32_t>(), plan_flags, out, out_stride, used);
     HAP_KLAUNCH(kStPlace, hap_place_fragments_kernel, dim3((unsigned)nfrag), dim3(kPlaceThreads), 0, st, G, base,
                 scratch.as<uint8_t>(), fsize.as<uint32_t>(), fdst.as<uint32_t>(), fidx.as<uint32_t>(),
                 write_index ? fent.as<uint8_t>() : (const uint8_t *)nullptr, out, out_stride);

@@ -10,6 +10,8 @@
 //   hap_place_fragments_kernel  one CTA per fragment: copies its element stream (or its raw DXT bytes
 //                            on a fallback) to the final position.  Chunks end up back to back with no
 //                            padding, exactly as hap.c:473 lays them out.
+// Behind the fused Hap Q encoder that writes its streams into the frames itself (hapq_fused_place_kernel), the plan
+// kernel's twin hap_plan_placed_frames_kernel lists the raw fragments instead, and hap_place_listed_kernel copies them.
 #pragma once
 #include "block_primitives.cuh"
 #include "hap_wire.h"
@@ -57,16 +59,29 @@ __device__ __forceinline__ uint32_t plan_excl_sum(uint32_t v, uint64_t *total, u
     return el + (eh << 16);
 }
 
+// What the fused Hap Q encoder that writes its streams into the frames (hapq_fused.cuh, hapq_fused_place_kernel) leaves
+// to the plan kernel: the stream bytes at or past the end a verbatim section would have (they wait in the fragment's
+// scratch slot, at their offset in the stream), the fragments' index entries, and a list of the fragments whose raw bytes
+// the place kernel must copy (work[0 .. *work_count)).
+struct PlanPlaced {
+    const uint8_t *scratch;        // [nfrag][kFragCap]
+    const uint8_t *frag_entries;   // [nfrag][kFragEntryStride] or nullptr
+    uint32_t *work, *work_count;
+};
+
 // out: [frames][out_stride]; frag_size / frag_dst / frag_idx_dst: [frames][G.frags_per_frame]; out_used: [frames].
 // flags & kPlanWriteIndex: a frame with at least one compressed chunk gets the trailing fragment index section
 // (hap_index.h); frag_idx_dst[f] then says where fragment f's entries go (0: nowhere).
 // flags & kPlanWriteOffsets: Complex sections carry the optional Chunk Offset Table (HapVideoDRAFT.md:126-128, honoured by
 // hap.c:697-700 and :800-803) and every chunk starts on a 16-byte boundary of the frame; the up to 15 bytes between two
 // chunks are zero.  The reference's own encoder never writes this table (hap.c:430-442), hence an option.
-__global__ void __launch_bounds__(kPlanThreads) hap_plan_frames_kernel(
-    FrameGeom G, const uint8_t *__restrict__ dxt, const uint32_t *__restrict__ frag_size,
+// PLACED: the compressed fragments are already in the frames (PlanPlaced above; no offset table): compressed fragments get
+// no destination, raw ones are listed for the place kernel.
+template <bool PLACED>
+__device__ __forceinline__ void plan_frames(
+    const FrameGeom &G, const uint8_t *__restrict__ dxt, const uint32_t *__restrict__ frag_size,
     uint32_t *__restrict__ frag_dst, uint32_t *__restrict__ frag_idx_dst, uint32_t flags, uint8_t *__restrict__ out,
-    uint64_t out_stride, unsigned long long *__restrict__ out_used)
+    uint64_t out_stride, unsigned long long *__restrict__ out_used, const PlanPlaced &pp)
 {
     __shared__ uint32_t scratch[kPlanThreads / 32];
     const uint32_t write_index = flags & kPlanWriteIndex, write_offsets = flags & kPlanWriteOffsets;
@@ -137,6 +152,7 @@ __global__ void __launch_bounds__(kPlanThreads) hap_plan_frames_kernel(
         uint32_t *fi = fi_frame + sec.frag_base;
         uint8_t *so = fo + sec_off[si];
         uint8_t *slots = ibody + kIndexHeaderBytes + 4u * (si ? k0 : 0u);   // this texture's record offsets
+        const uint32_t verbatim_end = sec_off[si] + hdr + sec.bytes;   // where the section would end stored verbatim (hap.c:490-495)
         if (complex_storage[si]) {
             uint8_t *p = so + hdr;
             uint8_t *ctab = p + 8, *stab = p + 8 + k + 4, *otab = stab + 4u * k + 4;
@@ -174,7 +190,13 @@ __global__ void __launch_bounds__(kPlanThreads) hap_plan_frames_kernel(
                         uint32_t eo = rec_off + 2u * fpc;   // entries follow the u16 sizes of the record
                         for (uint32_t j = 0; j < fpc; j++) {
                             const uint32_t s = fs[(uint64_t)c * fpc + j];
-                            fd[(uint64_t)c * fpc + j] = o;
+                            if (!PLACED) {
+                                fd[(uint64_t)c * fpc + j] = o;
+                            } else if (o + s > verbatim_end) {
+                                // the bytes the fused encoder kept back (fewer than top_hdr: the section is complex)
+                                const uint8_t *ks = pp.scratch + ((uint64_t)frame * G.frags_per_frame + sec.frag_base + (uint64_t)c * fpc + j) * kFragCap;
+                                for (uint32_t q = o > verbatim_end ? o : verbatim_end; q < o + s; q++) fo[q] = ks[q - o];
+                            }
                             o += s;
                             if (rec) {
                                 ibody[rec_off + 2 * j] = (uint8_t)s;
@@ -185,6 +207,10 @@ __global__ void __launch_bounds__(kPlanThreads) hap_plan_frames_kernel(
                         }
                     } else {
                         for (uint32_t j = 0; j < fpc; j++) fd[(uint64_t)c * fpc + j] = (start + j * kFragBytes) | kPlaceRawFlag;
+                        if (PLACED) {
+                            const uint32_t w = atomicAdd(pp.work_count, fpc);
+                            for (uint32_t j = 0; j < fpc; j++) pp.work[w + j] = frame * G.frags_per_frame + sec.frag_base + c * fpc + j;
+                        }
                     }
                 }
                 running += (uint32_t)ts;
@@ -199,10 +225,29 @@ __global__ void __launch_bounds__(kPlanThreads) hap_plan_frames_kernel(
                 uint32_t c = (uint32_t)(i / fpc), j = (uint32_t)(i % fpc);
                 fd[i] = (data0 + c * sec.chunk_bytes + j * kFragBytes) | kPlaceRawFlag;
             }
+            if (PLACED) {
+                __shared__ uint32_t work_base;
+                if (t == 0) work_base = atomicAdd(pp.work_count, k * fpc);
+                __syncthreads();
+                for (uint32_t i = t; i < k * fpc; i += kPlanThreads) pp.work[work_base + i] = frame * G.frags_per_frame + sec.frag_base + i;
+                __syncthreads();   // (work_base is taken again by the next section)
+            }
             // bytes / chunks truncates (hap.c:433); the verbatim path still copies every byte (hap.c:492)
             const uint32_t covered = k * sec.chunk_bytes;
             const uint8_t *in = dxt + (uint64_t)frame * sec.in_stride + sec.in_offset;
             for (uint32_t i = covered + t; i < sec.bytes; i += kPlanThreads) fo[data0 + i] = in[i];
+        }
+    }
+    if (PLACED && index_len) {
+        // the compressed fragments' index entries (a warp per fragment; frag_idx_dst was written by other threads)
+        __syncthreads();
+        const uint32_t lane = t & 31;
+        for (uint32_t f = t >> 5; f < G.frags_per_frame; f += kPlanThreads / 32) {
+            const uint32_t id = fi_frame[f];
+            if (id == 0) continue;
+            const uint8_t *e = pp.frag_entries + ((uint64_t)frame * G.frags_per_frame + f) * kFragEntryStride;
+            const uint32_t pieces = (fs_frame[f] + (1u << kIndexSubLog2) - 1u) >> kIndexSubLog2;
+            for (uint32_t q = lane; q < pieces; q += 32) fo[id + q] = e[q];
         }
     }
     if (t == 0) {
@@ -211,16 +256,32 @@ __global__ void __launch_bounds__(kPlanThreads) hap_plan_frames_kernel(
     }
 }
 
+__global__ void __launch_bounds__(kPlanThreads) hap_plan_frames_kernel(
+    FrameGeom G, const uint8_t *__restrict__ dxt, const uint32_t *__restrict__ frag_size,
+    uint32_t *__restrict__ frag_dst, uint32_t *__restrict__ frag_idx_dst, uint32_t flags, uint8_t *__restrict__ out,
+    uint64_t out_stride, unsigned long long *__restrict__ out_used)
+{
+    plan_frames<false>(G, dxt, frag_size, frag_dst, frag_idx_dst, flags, out, out_stride, out_used, PlanPlaced{});
+}
+
+// The plan kernel behind hapq_fused_place_kernel (flags without kPlanWriteOffsets).
+__global__ void __launch_bounds__(kPlanThreads) hap_plan_placed_frames_kernel(
+    FrameGeom G, const uint8_t *__restrict__ dxt, const uint32_t *__restrict__ frag_size,
+    uint32_t *__restrict__ frag_dst, uint32_t *__restrict__ frag_idx_dst, uint32_t flags, uint8_t *__restrict__ out,
+    uint64_t out_stride, unsigned long long *__restrict__ out_used, PlanPlaced pp)
+{
+    plan_frames<true>(G, dxt, frag_size, frag_dst, frag_idx_dst, flags, out, out_stride, out_used, pp);
+}
+
 constexpr int kPlaceThreads = 256;
 
-// grid.x = frames * frags_per_frame
-__global__ void __launch_bounds__(kPlaceThreads) hap_place_fragments_kernel(
-    FrameGeom G, const uint8_t *__restrict__ dxt, const uint8_t *__restrict__ scratch,
+// One fragment's bytes to their place in the frame: its element stream from scratch, or its raw bytes on a fallback.
+__device__ __forceinline__ void place_fragment(
+    uint32_t gfrag, const FrameGeom &G, const uint8_t *__restrict__ dxt, const uint8_t *__restrict__ scratch,
     const uint32_t *__restrict__ frag_size, const uint32_t *__restrict__ frag_dst, const uint32_t *__restrict__ frag_idx_dst,
     const uint8_t *__restrict__ frag_entries, uint8_t *__restrict__ out, uint64_t out_stride)
 {
     const int t = threadIdx.x;
-    const uint32_t gfrag = blockIdx.x;
     const uint32_t frame = gfrag / G.frags_per_frame;
     const uint32_t f = gfrag % G.frags_per_frame;
     const SectionGeom &sec = (G.sections == 2 && f >= G.s[1].frag_base) ? G.s[1] : G.s[0];
@@ -280,6 +341,26 @@ __global__ void __launch_bounds__(kPlaceThreads) hap_place_fragments_kernel(
     }
     const uint32_t done = head + (ng << 4);
     if ((uint32_t)t < n - done) dst[done + t] = src[done + t];
+}
+
+// grid.x = frames * frags_per_frame
+__global__ void __launch_bounds__(kPlaceThreads) hap_place_fragments_kernel(
+    FrameGeom G, const uint8_t *__restrict__ dxt, const uint8_t *__restrict__ scratch,
+    const uint32_t *__restrict__ frag_size, const uint32_t *__restrict__ frag_dst, const uint32_t *__restrict__ frag_idx_dst,
+    const uint8_t *__restrict__ frag_entries, uint8_t *__restrict__ out, uint64_t out_stride)
+{
+    place_fragment(blockIdx.x, G, dxt, scratch, frag_size, frag_dst, frag_idx_dst, frag_entries, out, out_stride);
+}
+
+// The raw fragments hap_plan_placed_frames_kernel listed (work[0 .. *work_count)), a persistent grid striding over them: on
+// content that compresses the list is empty and the launch costs next to nothing.
+__global__ void __launch_bounds__(kPlaceThreads) hap_place_listed_kernel(
+    FrameGeom G, const uint8_t *__restrict__ dxt, const uint32_t *__restrict__ frag_size, const uint32_t *__restrict__ frag_dst,
+    const uint32_t *__restrict__ work, const uint32_t *__restrict__ work_count, uint8_t *__restrict__ out, uint64_t out_stride)
+{
+    const uint32_t n = *work_count;
+    for (uint32_t i = blockIdx.x; i < n; i += gridDim.x)
+        place_fragment(work[i], G, dxt, nullptr, frag_size, frag_dst, nullptr, nullptr, out, out_stride);
 }
 
 }  // namespace hapb200

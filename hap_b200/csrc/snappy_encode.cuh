@@ -57,6 +57,7 @@ struct EncodeSmem {
     uint32_t entry[kFragEntryStride];               // fragment index: offset of the first element start in every 128 bytes of the stream
     uint32_t total;
     alignas(16) uint32_t out[(kFragCap + 3) / 4 + 6];   // the element stream (copied out in 16-byte words)
+    uint32_t place[6];                              // hapq_fused_place_kernel: ticket and the fragment waiting in `out`
 };
 // Two CTAs per SM: an H100 SM has 228 KiB of shared memory for CTAs and reserves 1 KiB of it per CTA, so each of two CTAs
 // may use (233,472 - 2 x 1,024) / 2 = 115,712 bytes.

@@ -17,6 +17,7 @@
 #include "hapq_fused.cuh"
 #include "snappy_decode.cuh"
 #include "snappy_encode.cuh"
+#include "yuv_sink.cuh"
 
 #include <atomic>
 #include <cstdio>
@@ -572,6 +573,44 @@ uint32_t launch_block_decode(const uint8_t *blocks, const uint8_t *alpha, uint32
     return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
 }
 
+// The NV12 / P010 sink of K8 (yuv_sink.cuh): blocks -> luma and chroma planes, frame f's at luma / chroma + f*frame_stride.
+// Launches count as bc_decode.  Hap Q Alpha decodes its YCoCg texture only: alpha is dropped.
+template <int KIND, int LAYOUT>
+void launch_bc_decode_yuv(uint32_t frames, cudaStream_t st, const uint8_t *blocks, const YuvOutGeom &g, uint8_t *luma, uint8_t *chroma,
+                          const uint32_t *frame_results)
+{
+    for (uint32_t f0 = 0; f0 < frames; f0 += kBcFramesPerLaunch) {
+        const dim3 grid((unsigned)yuv_out_ctas(g), frames - f0 < kBcFramesPerLaunch ? frames - f0 : kBcFramesPerLaunch);
+        HAP_KLAUNCH(kStBcDecode, (bc_decode_yuv_kernel<KIND, LAYOUT>), grid, dim3(kBcThreads), 0, st, blocks + f0 * g.in_stride, g,
+                    luma + f0 * g.frame_bytes, chroma + f0 * g.frame_bytes, frame_results ? frame_results + f0 : nullptr);
+    }
+}
+
+template <int KIND>
+void launch_bc_decode_yuv_layout(uint32_t frames, cudaStream_t st, const uint8_t *blocks, const YuvOutGeom &g, uint8_t *luma, uint8_t *chroma,
+                                 unsigned layout, const uint32_t *frame_results)
+{
+    if (layout == HapB200YUV_P010) launch_bc_decode_yuv<KIND, HapB200YUV_P010>(frames, st, blocks, g, luma, chroma, frame_results);
+    else launch_bc_decode_yuv<KIND, HapB200YUV_NV12>(frames, st, blocks, g, luma, chroma, frame_results);
+}
+
+uint32_t launch_block_decode_yuv(const uint8_t *blocks, uint32_t frames, uint64_t blocks_stride, uint32_t width, uint32_t height,
+                                 const CodecInfo &ci, uint8_t *luma, uint8_t *chroma, uint64_t frame_stride, uint64_t pitch, unsigned layout,
+                                 unsigned color_space, cudaStream_t st, const uint32_t *frame_results = nullptr)
+{
+    const YuvOutGeom g = yuv_out_geom(width, height, (uint32_t)pitch, blocks_stride, frame_stride, layout, color_space);   // (pitch < 2^32)
+    switch (ci.bc_kind) {
+    case kBcDxt1: launch_bc_decode_yuv_layout<kBcDxt1>(frames, st, blocks, g, luma, chroma, layout, frame_results); break;
+    case kBcDxt5: launch_bc_decode_yuv_layout<kBcDxt5>(frames, st, blocks, g, luma, chroma, layout, frame_results); break;
+    case kBcRgtc1: launch_bc_decode_yuv_layout<kBcRgtc1>(frames, st, blocks, g, luma, chroma, layout, frame_results); break;
+    case kBcYCoCg:
+    case kBcYCoCgPlusAlpha: launch_bc_decode_yuv_layout<kBcYCoCg>(frames, st, blocks, g, luma, chroma, layout, frame_results); break;
+    case kBcBc7: launch_bc_decode_yuv_layout<kBcBc7>(frames, st, blocks, g, luma, chroma, layout, frame_results); break;
+    default: return HapResult_Internal_Error;
+    }
+    return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
+}
+
 // BC6H (Hap HDR) blocks -> RGBA16F.  Signedness per frame from frame_formats, or is_signed for all.  One launch per
 // kBcFramesPerLaunch frames.
 uint32_t launch_bc6h_decode(const uint8_t *blocks, uint32_t frames, uint64_t blocks_stride, uint32_t width, uint32_t height, uint8_t *rgba,
@@ -752,20 +791,22 @@ __global__ void ring_wait_kernel(const unsigned int *flag, unsigned int value, u
 }
 }  // namespace
 
-// The single-frame picture decoders (HapB200DecodeRGBA, HapB200DecodeRGBAHalf): textures 0 .. count-1 of the frame, t[i]
-// bytes each, are decoded by HapDecode into device scratch (a texture that does not fill its room: Bad_Frame); then
-// launch(textures, picture, tight row bytes, stream) writes a tight picture of bpp bytes per pixel, which is copied to the
-// caller's rows.
+// The single-frame picture decoders (HapB200DecodeRGBA, HapB200DecodeRGBAHalf, HapB200DecodeYUV): textures 0 .. count-1 of
+// the frame, t[i] bytes each, are decoded by HapDecode into device scratch (a texture that does not fill its room: Bad_Frame);
+// then launch(textures, picture, tight row bytes, stream) writes a tight picture of bpp bytes per pixel, which is copied to the
+// caller's rows.  With a `chroma` plane the picture has a second plane of height/2 rows of the same width, which launch writes
+// at picture + tight * height and which is copied to chroma's rows (rowBytes apart, as the first plane's).
 template <class Launch>
 uint32_t decode_frame_to_picture(const void *inputBuffer, unsigned long inputBufferBytes, unsigned count, const uint64_t t[2],
-                                 unsigned width, unsigned height, uint64_t bpp, void *picture, unsigned long rowBytes, Launch &&launch)
+                                 unsigned width, unsigned height, uint64_t bpp, void *picture, unsigned long rowBytes, Launch &&launch,
+                                 void *chroma = nullptr)
 {
-    HAP_ENTER(inputBuffer, picture);
-    const uint64_t tight = bpp * width;
+    HAP_ENTER(inputBuffer, picture, chroma);
+    const uint64_t tight = bpp * width, first = tight * height, second = chroma ? tight * (height / 2) : 0;
     // scratch from the device's stream-ordered pool on the legacy stream (the nested HapDecode calls below write it on
     // that stream, or on a pooled stream they synchronise before returning): no cudaMalloc/cudaFree, no device-wide sync
     DevBuf texb(kLegacyStream), imgb(kLegacyStream);
-    if (!texb.alloc(align16(t[0]) + align16(t[1]) + 16) || !imgb.alloc(tight * height)) { cudaGetLastError(); return HapResult_Internal_Error; }
+    if (!texb.alloc(align16(t[0]) + align16(t[1]) + 16) || !imgb.alloc(first + second)) { cudaGetLastError(); return HapResult_Internal_Error; }
     if (cudaStreamSynchronize(kLegacyStream) != cudaSuccess) { cudaGetLastError(); return HapResult_Internal_Error; }   // the allocations are real now
     auto serial = [](HapDecodeWorkFunction fn, void *p, unsigned n, void *) { for (unsigned i = 0; i < n; i++) fn(p, i); };
     uint32_t r = HapResult_No_Error;
@@ -781,6 +822,7 @@ uint32_t decode_frame_to_picture(const void *inputBuffer, unsigned long inputBuf
         r = launch((const uint8_t *)texb.p, imgb.as<uint8_t>(), tight, st);
         if (r == HapResult_No_Error &&
             (cudaMemcpy2DAsync(picture, rowBytes, imgb.p, tight, tight, height, cudaMemcpyDefault, st) != cudaSuccess ||
+             (chroma && cudaMemcpy2DAsync(chroma, rowBytes, imgb.as<uint8_t>() + first, tight, tight, height / 2, cudaMemcpyDefault, st) != cudaSuccess) ||
              cudaStreamSynchronize(st) != cudaSuccess)) { cudaGetLastError(); r = HapResult_Internal_Error; }
     }
     return r;
@@ -1522,6 +1564,33 @@ unsigned int HapB200DecodeBatch(const void *in, unsigned int frames, unsigned lo
     });
 }
 
+// The texture half of the picture batch decoders (HapB200DecodeRGBABatch, HapB200DecodeYUVBatch): every texture of every frame
+// decoded into device scratch `dxt`, allocated here (frame f at f * (align16(t[0]) + align16(t[1])), texture 1 at align16(t[0])
+// inside it), and results[f] set as HapB200DecodeRGBABatch reports it.
+static uint32_t decode_textures_batch(const void *in, unsigned frames, unsigned long inStride, const unsigned long long *inBytes,
+                                      unsigned maxChunks, const CodecInfo &ci, const uint64_t t[2], DevBuf &dxt, unsigned *results,
+                                      cudaStream_t st)
+{
+    const uint64_t dxt_stride = align16(t[0]) + align16(t[1]);
+    DevBuf used(st), formats(st), res1(st);
+    if (!dxt.alloc(dxt_stride * frames + 16) || !used.alloc(8ull * frames) || !formats.alloc(4ull * frames) || !res1.alloc(4ull * frames)) {
+        cudaGetLastError();
+        return HapResult_Internal_Error;
+    }
+    for (uint32_t ti = 0; ti < ci.textures; ti++) {
+        uint32_t *res = ti == 0 ? results : res1.as<uint32_t>();
+        // the decoded size must equal the texture size: offer exactly that much room per frame (the slot stride is
+        // wider: both textures of a frame share a slot, so a texture that over-declares its size must not reach its
+        // neighbour or the next frame's slot)
+        const uint32_t r = launch_decode_batch((const uint8_t *)in, frames, inStride, inBytes, ti, maxChunks, dxt.as<uint8_t>() + (ti ? align16(t[0]) : 0),
+                                               dxt_stride, t[ti], used.as<unsigned long long>(), formats.as<uint32_t>(), res, st);
+        if (r != HapResult_No_Error) return r;
+        HAP_KLAUNCH(kStCollect, hap_check_texture_kernel, dim3((frames + 127) / 128), dim3(128), 0, st, frames, used.as<unsigned long long>(),
+                    formats.as<uint32_t>(), res, (unsigned long long)t[ti], ci.fmt[ti], results);
+    }
+    return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
+}
+
 unsigned int HapB200DecodeRGBABatch(const void *in, unsigned int frames, unsigned long inStride, const unsigned long long *inBytes,
                                     unsigned int maxChunks, unsigned int codec, unsigned int width, unsigned int height, void *rgba,
                                     unsigned long frameStride, unsigned long rowBytes, unsigned int *results, void *stream)
@@ -1532,33 +1601,19 @@ unsigned int HapB200DecodeRGBABatch(const void *in, unsigned int frames, unsigne
         return HapResult_Bad_Arguments;
     HAP_ENTER(in, rgba);
     return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
-        const uint64_t t0 = HapB200TextureBytes(width, height, codec, 0), t1 = HapB200TextureBytes(width, height, codec, 1);
-        const uint64_t dxt_stride = align16(t0) + align16(t1);
-        DevBuf dxt(st), used(st), formats(st), res1(st);
-        if (!dxt.alloc(dxt_stride * frames + 16) || !used.alloc(8ull * frames) || !formats.alloc(4ull * frames) || !res1.alloc(4ull * frames)) {
-            cudaGetLastError();
-            return HapResult_Internal_Error;
-        }
-        for (uint32_t ti = 0; ti < ci.textures; ti++) {
-            uint32_t *res = ti == 0 ? results : res1.as<uint32_t>();
-            // the decoded size must equal the texture size: offer exactly that much room per frame (the slot stride is
-            // wider: both textures of a frame share a slot, so a texture that over-declares its size must not reach its
-            // neighbour or the next frame's slot)
-            const uint32_t r = launch_decode_batch((const uint8_t *)in, frames, inStride, inBytes, ti, maxChunks, dxt.as<uint8_t>() + (ti ? align16(t0) : 0),
-                                                   dxt_stride, ti ? t1 : t0, used.as<unsigned long long>(), formats.as<uint32_t>(), res, st);
-            if (r != HapResult_No_Error) return r;
-            HAP_KLAUNCH(kStCollect, hap_check_texture_kernel, dim3((frames + 127) / 128), dim3(128), 0, st, frames, used.as<unsigned long long>(),
-                        formats.as<uint32_t>(), res, (unsigned long long)(ti ? t1 : t0), ci.fmt[ti], results);
-        }
-        return launch_block_decode(dxt.as<uint8_t>(), dxt.as<uint8_t>() + align16(t0), frames, dxt_stride, dxt_stride, width, height, ci,
-                                   (uint8_t *)rgba, frameStride, rowBytes, st, results);
+        const uint64_t t[2] = {texture_bytes(width, height, ci, 0), texture_bytes(width, height, ci, 1)};
+        DevBuf dxt(st);
+        const uint32_t r = decode_textures_batch(in, frames, inStride, inBytes, maxChunks, ci, t, dxt, results, st);
+        if (r != HapResult_No_Error) return r;
+        return launch_block_decode(dxt.as<uint8_t>(), dxt.as<uint8_t>() + align16(t[0]), frames, align16(t[0]) + align16(t[1]),
+                                   align16(t[0]) + align16(t[1]), width, height, ci, (uint8_t *)rgba, frameStride, rowBytes, st, results);
     });
 }
 
-unsigned int HapB200DecodeRGBA(const void *inputBuffer, unsigned long inputBufferBytes, unsigned int width, unsigned int height,
-                               void *rgba, unsigned long rowBytes)
+// The codec whose textures a frame has (BC6H frames, Hap HDR, decode to half floats: HapB200DecodeRGBAHalf; Bad_Frame here),
+// for the single-frame RGBA8 and YUV decoders
+static uint32_t frame_codec(const void *inputBuffer, unsigned long inputBufferBytes, CodecInfo &ci)
 {
-    if (!inputBuffer || !rgba_geometry_ok(rgba, width, height, rowBytes, 0, false)) return HapResult_Bad_Arguments;
     unsigned count = 0, f0 = 0, f1 = 0;
     uint32_t r = HapGetFrameTextureCount(inputBuffer, inputBufferBytes, &count);
     if (r != HapResult_No_Error) return r;
@@ -1568,16 +1623,83 @@ unsigned int HapB200DecodeRGBA(const void *inputBuffer, unsigned long inputBuffe
         r = HapGetFrameTextureFormat(inputBuffer, inputBufferBytes, 1, &f1);
         if (r != HapResult_No_Error) return r;
     }
-    // the codec whose textures the frame has (BC6H frames, Hap HDR, decode to half floats: HapB200DecodeRGBAHalf; Bad_Frame here)
     unsigned codec = 0;
-    CodecInfo ci;
     while (codec_info(codec, ci) && (ci.textures != count || ci.fmt[0] != f0 || (count == 2 && ci.fmt[1] != f1))) codec++;
-    if (!codec_info(codec, ci)) return HapResult_Bad_Frame;
-    const uint64_t t[2] = {HapB200TextureBytes(width, height, codec, 0), HapB200TextureBytes(width, height, codec, 1)};
-    return decode_frame_to_picture(inputBuffer, inputBufferBytes, count, t, width, height, 4, rgba, rowBytes,
+    return codec_info(codec, ci) ? HapResult_No_Error : HapResult_Bad_Frame;
+}
+
+unsigned int HapB200DecodeRGBA(const void *inputBuffer, unsigned long inputBufferBytes, unsigned int width, unsigned int height,
+                               void *rgba, unsigned long rowBytes)
+{
+    if (!inputBuffer || !rgba_geometry_ok(rgba, width, height, rowBytes, 0, false)) return HapResult_Bad_Arguments;
+    CodecInfo ci;
+    const uint32_t r = frame_codec(inputBuffer, inputBufferBytes, ci);
+    if (r != HapResult_No_Error) return r;
+    const uint64_t t[2] = {texture_bytes(width, height, ci, 0), texture_bytes(width, height, ci, 1)};
+    return decode_frame_to_picture(inputBuffer, inputBufferBytes, ci.textures, t, width, height, 4, rgba, rowBytes,
                                    [&](const uint8_t *tex, uint8_t *img, uint64_t tight, cudaStream_t st) {
                                        return launch_block_decode(tex, tex + align16(t[0]), 1, 0, 0, width, height, ci, img, 0, tight, st);
                                    });
+}
+
+// ---- Hap, Hap Alpha, Hap Q, Hap Q Alpha, Hap Alpha-Only, Hap R -> NV12 / P010: K8 with a YUV sink (yuv_sink.cuh) ----------
+
+// the layouts and colour spaces the YUV decoders take (BT.601 / BT.709; no BT.2020)
+static bool yuv_out_args_ok(unsigned layout, unsigned colorSpace) { return layout <= HapB200YUV_P010 && colorSpace <= HapB200YUV_BT709_Full; }
+
+static uint64_t yuv_sample_bytes(unsigned layout) { return layout == HapB200YUV_P010 ? 2 : 1; }
+
+unsigned int HapB200BlockDecodeYUVBatch(const void *blocks, unsigned int frames, unsigned long blocksStride, unsigned int width,
+                                        unsigned int height, unsigned int codec, void *luma, void *chroma, unsigned long frameStride,
+                                        unsigned long pitch, unsigned int layout, unsigned int colorSpace, void *stream)
+{
+    CodecInfo ci;
+    if (!blocks || frames == 0 || !codec_info(codec, ci) || !yuv_out_args_ok(layout, colorSpace) ||
+        !yuv_geometry_ok(luma, chroma, width, height, pitch, frameStride, true, yuv_sample_bytes(layout)) || ((uintptr_t)blocks | blocksStride) % 16)
+        return HapResult_Bad_Arguments;
+    HAP_ENTER(blocks, luma);
+    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
+        return launch_block_decode_yuv((const uint8_t *)blocks, frames, blocksStride, width, height, ci, (uint8_t *)luma, (uint8_t *)chroma,
+                                       frameStride, pitch, layout, colorSpace, st);
+    });
+}
+
+unsigned int HapB200DecodeYUVBatch(const void *in, unsigned int frames, unsigned long inStride, const unsigned long long *inBytes,
+                                   unsigned int maxChunks, unsigned int codec, unsigned int width, unsigned int height, void *luma,
+                                   void *chroma, unsigned long frameStride, unsigned long pitch, unsigned int layout, unsigned int colorSpace,
+                                   unsigned int *results, void *stream)
+{
+    CodecInfo ci;
+    if (!in || !inBytes || !results || frames == 0 || maxChunks == 0 || !codec_info(codec, ci) || !yuv_out_args_ok(layout, colorSpace) ||
+        !yuv_geometry_ok(luma, chroma, width, height, pitch, frameStride, true, yuv_sample_bytes(layout)))
+        return HapResult_Bad_Arguments;
+    HAP_ENTER(in, luma);
+    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
+        const uint64_t t[2] = {texture_bytes(width, height, ci, 0), texture_bytes(width, height, ci, 1)};
+        DevBuf dxt(st);
+        const uint32_t r = decode_textures_batch(in, frames, inStride, inBytes, maxChunks, ci, t, dxt, results, st);
+        if (r != HapResult_No_Error) return r;
+        return launch_block_decode_yuv(dxt.as<uint8_t>(), frames, align16(t[0]) + align16(t[1]), width, height, ci, (uint8_t *)luma,
+                                       (uint8_t *)chroma, frameStride, pitch, layout, colorSpace, st, results);
+    });
+}
+
+unsigned int HapB200DecodeYUV(const void *inputBuffer, unsigned long inputBufferBytes, unsigned int width, unsigned int height, void *luma,
+                              void *chroma, unsigned long pitch, unsigned int layout, unsigned int colorSpace)
+{
+    if (!inputBuffer || !yuv_out_args_ok(layout, colorSpace) ||
+        !yuv_geometry_ok(luma, chroma, width, height, pitch, 0, false, yuv_sample_bytes(layout)))
+        return HapResult_Bad_Arguments;
+    CodecInfo ci;
+    const uint32_t r = frame_codec(inputBuffer, inputBufferBytes, ci);
+    if (r != HapResult_No_Error) return r;
+    const uint64_t t[2] = {texture_bytes(width, height, ci, 0), texture_bytes(width, height, ci, 1)};
+    return decode_frame_to_picture(
+        inputBuffer, inputBufferBytes, ci.textures, t, width, height, yuv_sample_bytes(layout), luma, pitch,
+        [&](const uint8_t *tex, uint8_t *img, uint64_t tight, cudaStream_t st) {
+            return launch_block_decode_yuv(tex, 1, 0, width, height, ci, img, img + tight * height, 0, tight, layout, colorSpace, st);
+        },
+        chroma);
 }
 
 bool is_bc6h_format(unsigned f) { return f == HapFmt_RGB_BPTC_UFLOAT || f == HapFmt_RGB_BPTC_SFLOAT; }

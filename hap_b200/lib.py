@@ -86,6 +86,12 @@ class HapB200(HapABI):
         L.HapB200EncodeYUVBatch.argtypes = [vp, vp, u, ul, u, u, ul, u, u, u, u, u, vp, ul, vp, vp]
         L.HapB200BlockEncodeYUVBatch.restype = u
         L.HapB200BlockEncodeYUVBatch.argtypes = [vp, vp, u, ul, u, u, ul, u, u, u, vp, ul, vp]
+        L.HapB200DecodeYUV.restype = u
+        L.HapB200DecodeYUV.argtypes = [vp, ul, u, u, vp, vp, ul, u, u]
+        L.HapB200DecodeYUVBatch.restype = u
+        L.HapB200DecodeYUVBatch.argtypes = [vp, u, ul, vp, u, u, u, u, vp, vp, ul, ul, u, u, vp, vp]
+        L.HapB200BlockDecodeYUVBatch.restype = u
+        L.HapB200BlockDecodeYUVBatch.argtypes = [vp, u, ul, u, u, u, vp, vp, ul, ul, u, u, vp]
         L.HapB200EncodeYUVPQ.restype = u
         L.HapB200EncodeYUVPQ.argtypes = [vp, vp, u, u, ul, u, u, u, u, u, vp, ul, C.POINTER(ul)]
         L.HapB200EncodeYUVPQBatch.restype = u
@@ -315,6 +321,34 @@ class HapB200(HapABI):
                                blocks_stride, stream=None):
         return int(self.lib.HapB200BlockEncodeYUVBatch(luma, chroma, frames, frame_stride, w, h, pitch, layout, color_space, codec,
                                                        blocks, blocks_stride, stream))
+
+    # -- Hap (every codec but Hap HDR) -> NV12 / P010: layout HapB200YUV_*, color_space BT.601 / BT.709 (no BT.2020); both
+    #    planes have the row pitch `pitch` (default: width bytes per sample)
+    def decode_yuv(self, frame, w, h, layout, color_space, pitch=None, luma=None, chroma=None, frame_bytes=None):
+        """frame, luma, chroma: buffer objects or (addr, nbytes).  Returns (result, (luma bytes, chroma bytes)) when it
+        allocates the planes (luma and chroma not given), else (result, None)."""
+        from .abi import _as_ptr
+        faddr, fn = _as_ptr(frame)
+        if frame_bytes is not None:
+            fn = frame_bytes
+        pitch = pitch or (2 if layout == HapB200YUV_P010 else 1) * w
+        own = luma is None and chroma is None
+        if own:
+            luma, chroma = bytearray(pitch * h), bytearray(pitch * (h // 2))
+        laddr, _ = _as_ptr(luma)
+        caddr, _ = _as_ptr(chroma)
+        r = self.lib.HapB200DecodeYUV(faddr, fn, w, h, laddr, caddr, pitch, layout, color_space)
+        return int(r), ((bytes(luma), bytes(chroma)) if own and r == 0 else None)
+
+    def decode_yuv_batch(self, frames_ptr, frames, in_stride, in_bytes, max_chunks, codec, w, h, luma, chroma, frame_stride, pitch, layout,
+                         color_space, results, stream=None):
+        return int(self.lib.HapB200DecodeYUVBatch(frames_ptr, frames, in_stride, in_bytes, max_chunks, codec, w, h, luma, chroma, frame_stride,
+                                                  pitch, layout, color_space, results, stream))
+
+    def block_decode_yuv_batch(self, blocks, frames, blocks_stride, w, h, codec, luma, chroma, frame_stride, pitch, layout, color_space,
+                               stream=None):
+        return int(self.lib.HapB200BlockDecodeYUVBatch(blocks, frames, blocks_stride, w, h, codec, luma, chroma, frame_stride, pitch, layout,
+                                                       color_space, stream))
 
     # -- HDR10 P010 (BT.2020, PQ) -> Hap HDR (BC6H): color_space HapB200YUV_BT2020_*, unit_nits the cd/m2 of 1.0 (1-10000),
     #    texture_format UF16 or SF16; planes as for encode_yuv with HapB200YUV_P010 (pitch default 2 * width); frames need

@@ -325,6 +325,72 @@ unsigned int HapB200BlockEncodeYUVBatch(const void *luma, const void *chroma, un
                                         unsigned int colorSpace, unsigned int codec, void *blocks, unsigned long blocksStride,
                                         void *stream);
 
+/* ---- Hap, Hap Alpha, Hap Q, Hap Q Alpha, Hap Alpha-Only, Hap R -> NV12 / P010 ------------------------------------------------
+ * The decoders write the 4:2:0 pictures a video encoder takes (NVENC surfaces).  The conversion is fused into the block
+ * decoder, so no RGBA picture is ever written.  The planes are exactly the conversion below applied to the RGBA8 picture that
+ * HapB200DecodeRGBA / HapB200DecodeRGBABatch / HapB200BlockDecodeBatch give for the same input; alpha is ignored.
+ * Planes, pitch and layouts: those of the YUV encoders above (HapB200YUV_NV12: bytes; HapB200YUV_P010: little-endian 16-bit
+ * words holding sample << 6, the low 6 bits zero).  One pitch for both planes; chroma is a pointer of its own.  In a batch frame
+ * f's planes start at luma + f*frameStride and chroma + f*frameStride.  The only bytes written are the width * (bytes per
+ * sample) bytes of each of the height luma rows and height/2 chroma rows: pitch slack and whatever lies between planes and
+ * frames stays as it was.
+ * Geometry: that of the YUV encoders (width and height multiples of 4, width * (bytes per sample) <= pitch <=
+ * HAPB200_MAX_ROW_BYTES, at most HAPB200_MAX_BLOCKS blocks).  The batch entry points take device pointers; luma, chroma, pitch,
+ * frameStride, blocks and blocksStride are 16-byte aligned; a batch may hold any number of frames.  The single-frame call takes
+ * host or device pointers at any alignment and any pitch.
+ * Codecs: every HapB200Codec.  Hap Alpha-Only (HapA) decodes to (v, v, v, 255), so its matte comes out as a grey luma picture
+ * with neutral chroma: a key signal.  Colour spaces: BT.601 and BT.709, limited and full range; BT.2020 is refused with
+ * HapResult_Bad_Arguments (8-bit Hap into BT.2020 would be a gamut decision), as are an unknown layout or colour space.  Every
+ * argument is checked before anything touches the GPU.
+ * Results: HapB200DecodeYUV answers exactly as HapB200DecodeRGBA does (Hap HDR (BC6H) frames: HapResult_Bad_Frame);
+ * HapB200DecodeYUVBatch reports in results[f] exactly what HapB200DecodeRGBABatch reports.  A failed frame's RGBA picture is
+ * all zero bytes, so its planes are the conversion of zeros: black, Y = yOff and Cb = Cr = cOff.
+ * The conversion, exactly (n = 8 for NV12, 10 for P010; scales and offsets those of the encoders' definition: limited range
+ * luma offset 16 * 2^(n-8), luma scale 219 * 2^(n-8), chroma scale 224 * 2^(n-8); full range offset 0 and both scales
+ * 2^n - 1; chroma offset 2^(n-1)):
+ *   Coefficients: L = 65536 * lumaScale / 255 and S = 65536 * chromaScale / 255, (Kr, Kb) = BT.601 (0.299, 0.114) or BT.709
+ *   (0.2126, 0.0722), Kg = 1 - Kr - Kb, round() to nearest, halves up:
+ *     yR = round(L*Kr), yB = round(L*Kb), yG = round(L) - yR - yB;
+ *     cbR = round(-S*Kr / (2(1-Kb))), cbG = round(-S*Kg / (2(1-Kb))), cbB = -(cbR + cbG);
+ *     crG = round(-S*Kg / (2(1-Kr))), crB = round(-S*Kb / (2(1-Kr))), crR = -(crG + crB).
+ *   The derived entries make every grey map to exactly neutral chroma, and 0 and 255 to the nominal black and white codes.
+ *   They are the rows of HAPB200_YUV_OUT_COEFFICIENTS below.
+ *   Luma, per pixel: Y = ((yR*R + yG*G + yB*B + 32768) >> 16) + yOff, clamped to 0..2^n-1.
+ *   Chroma, 4:2:0 at the default siting the encoders' upsampler assumes (chroma_sample_loc_type 0: co-sited with even luma
+ *   columns, midway between luma rows 2j and 2j+1): for chroma sample (i, j), Rs, Gs and Bs are the sums of R, G and B over
+ *   luma columns 2i-1, 2i, 2i+1 with weights 1, 2, 1 (column -1 clamped to 0) and rows 2j and 2j+1 with weight 1 each, a
+ *   total weight of 8; then
+ *     Cb = ((cbR*Rs + cbG*Gs + cbB*Bs + 2^18) >> 19) + cOff,  Cr = ((crR*Rs + crG*Gs + crB*Bs + 2^18) >> 19) + cOff,
+ *   the shift arithmetic, each clamped to 0..2^n-1.  Every intermediate is below 2^31.
+ *   A flat colour converted to P010 here and back by the YUV encoders' conversion returns exactly, for all 2^24 colours. */
+/* row layout * 4 + colorSpace: {yR, yG, yB, cbR, cbG, cbB, crR, crG, crB, yOff, cOff} */
+#define HAPB200_YUV_OUT_COEFFICIENTS                                                                                       \
+    {                                                                                                                      \
+        {16829, 33039, 6416, -9714, -19071, 28785, 28784, -24103, -4681, 16, 128},        /* NV12 BT.601 limited */        \
+        {19595, 38470, 7471, -11058, -21710, 32768, 32768, -27439, -5329, 0, 128},        /* NV12 BT.601 full    */        \
+        {11966, 40254, 4064, -6596, -22189, 28785, 28784, -26145, -2639, 16, 128},        /* NV12 BT.709 limited */        \
+        {13933, 46871, 4732, -7509, -25259, 32768, 32768, -29763, -3005, 0, 128},         /* NV12 BT.709 full    */        \
+        {67315, 132155, 25665, -38856, -76282, 115138, 115137, -96413, -18724, 64, 512},  /* P010 BT.601 limited */        \
+        {78612, 154331, 29972, -44363, -87094, 131457, 131457, -110079, -21378, 0, 512},  /* P010 BT.601 full    */        \
+        {47864, 161016, 16255, -26383, -88755, 115138, 115137, -104580, -10557, 64, 512}, /* P010 BT.709 limited */        \
+        {55896, 188037, 18982, -30123, -101335, 131458, 131458, -119404, -12054, 0, 512}  /* P010 BT.709 full    */        \
+    }
+
+/* one Hap frame (host or device pointers, any alignment) -> one NV12 / P010 picture */
+unsigned int HapB200DecodeYUV(const void *inputBuffer, unsigned long inputBufferBytes, unsigned int width, unsigned int height,
+                              void *luma, void *chroma, unsigned long pitch, unsigned int layout, unsigned int colorSpace);
+/* frames x Hap frame (device, as HapB200DecodeRGBABatch) -> frames x picture (device): frame f's planes at luma + f*frameStride,
+ * chroma + f*frameStride */
+unsigned int HapB200DecodeYUVBatch(const void *in, unsigned int frames, unsigned long inStride, const unsigned long long *inBytes,
+                                   unsigned int maxChunks, unsigned int codec, unsigned int width, unsigned int height,
+                                   void *luma, void *chroma, unsigned long frameStride, unsigned long pitch,
+                                   unsigned int layout, unsigned int colorSpace, unsigned int *results, void *stream);
+/* bare textures (device, as HapB200BlockDecodeBatch; HapM: the RGTC1 plane at blocks + HapB200TextureBytes(.., 0), which is
+ * not read, alpha being dropped) -> pictures */
+unsigned int HapB200BlockDecodeYUVBatch(const void *blocks, unsigned int frames, unsigned long blocksStride, unsigned int width,
+                                        unsigned int height, unsigned int codec, void *luma, void *chroma, unsigned long frameStride,
+                                        unsigned long pitch, unsigned int layout, unsigned int colorSpace, void *stream);
+
 /* ---- Hap HDR (BC6H, "HapH") <- HDR10 P010 (BT.2020, SMPTE ST 2084 / PQ) --------------------------------------------------
  * The encoders take the P010 pictures a video decoder writes for HEVC Main10 HDR10 and convert them to linear RGBA16F inside
  * the BC6H encoder, so no RGBA16F picture is ever written.  A P010 picture encodes to exactly the bytes

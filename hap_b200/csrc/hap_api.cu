@@ -440,23 +440,28 @@ uint32_t launch_block_encode(const uint8_t *rgba, uint32_t frames, uint64_t fram
     return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
 }
 
-// The PQ tables of the HDR10 encoders: T of include/hap_b200.h per (device, unitNits), built on the host (yuv_pq_table) and
-// uploaded by the first call that needs it, which waits for the copy; 8 KiB each, kept for the life of the process, so later
-// calls (batches among them) find it without touching the host.  nullptr when the upload fails.
-const uint16_t *pq_table(uint32_t unit_nits)
+// The PQ tables of the HDR10 converters per (device, direction, unitNits): T of the encoders (kPqIn: yuv_pq_table, 4096
+// halves, 8 KiB) and P of the decoders (kPqOut: yuv_pq_out_table, kPqOutEntries codes, 62 KiB), both of include/hap_b200.h.
+// Built on the host and uploaded by the first call that needs one, which waits for the copy; kept for the life of the
+// process, so later calls (batches among them) find it without touching the host.  nullptr when the upload fails.
+enum PqDirection : uint32_t { kPqIn = 0, kPqOut = 1 };
+const uint16_t *pq_table(uint32_t unit_nits, PqDirection dir)
 {
     static std::mutex mu;
     static std::map<uint32_t, uint16_t *> tables[kMaxDevices];
     std::lock_guard<std::mutex> l(mu);
     std::map<uint32_t, uint16_t *> &mine = tables[t_device];
-    const auto it = mine.find(unit_nits);
+    const uint32_t key = unit_nits << 1 | dir;
+    const auto it = mine.find(key);
     if (it != mine.end()) return it->second;
-    std::vector<uint16_t> host(4096);
-    yuv_pq_table(unit_nits, host.data());
+    const size_t bytes = (dir == kPqOut ? kPqOutEntries : 4096) * sizeof(uint16_t);
+    std::vector<uint16_t> host(bytes / sizeof(uint16_t));
+    if (dir == kPqOut) yuv_pq_out_table(unit_nits, host.data());
+    else yuv_pq_table(unit_nits, host.data());
     void *d = nullptr;
     cudaStream_t s = nullptr;
-    bool ok = cudaMalloc(&d, 4096 * sizeof(uint16_t)) == cudaSuccess && cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking) == cudaSuccess;
-    ok = ok && cudaMemcpyAsync(d, host.data(), 4096 * sizeof(uint16_t), cudaMemcpyHostToDevice, s) == cudaSuccess;
+    bool ok = cudaMalloc(&d, bytes) == cudaSuccess && cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking) == cudaSuccess;
+    ok = ok && cudaMemcpyAsync(d, host.data(), bytes, cudaMemcpyHostToDevice, s) == cudaSuccess;
     ok = ok && cudaStreamSynchronize(s) == cudaSuccess;
     if (s) cudaStreamDestroy(s);
     if (!ok) {
@@ -464,7 +469,7 @@ const uint16_t *pq_table(uint32_t unit_nits)
         if (d) cudaFree(d);
         return nullptr;
     }
-    return mine[unit_nits] = (uint16_t *)d;
+    return mine[key] = (uint16_t *)d;
 }
 
 // The picture an encoder reads: an RGBA8 picture (kSrcRgba8), the luma and chroma planes of an NV12 / P010 picture
@@ -497,7 +502,7 @@ uint32_t launch_bc6h_encode(const PictureSrc &p, uint32_t frames, uint64_t frame
     const BcGeom g = bc_encode_geom(width, height, (uint32_t)row_bytes, frame_stride, blocks_stride, 0);   // (rgba_geometry_ok: row_bytes < 2^32)
     YuvPqSrc pq = YuvPqSrc();
     if (p.kind == kSrcP010Pq) {
-        const uint16_t *table = pq_table(p.unit_nits);
+        const uint16_t *table = pq_table(p.unit_nits, kPqIn);
         if (!table) return HapResult_Internal_Error;
         pq = yuv_pq_src(p.color_space, (const uint8_t *)p.chroma, table);
     }
@@ -622,6 +627,25 @@ uint32_t launch_bc6h_decode(const uint8_t *blocks, uint32_t frames, uint64_t blo
         const dim3 grid(bc_ctas(g.blocks_x, g.blocks_y), frames - f0 < kBcFramesPerLaunch ? frames - f0 : kBcFramesPerLaunch);
         HAP_KLAUNCH(kStBcDecode, bc6h_decode_kernel, grid, dim3(kBcThreads), 0, st, blocks + f0 * g.in_stride, g, rgba + f0 * g.frame_bytes,
                     frame_results ? frame_results + f0 : nullptr, frame_formats ? frame_formats + f0 : nullptr, is_signed ? 1u : 0u);
+    }
+    return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
+}
+
+// The HDR10 sink of K8 (yuv_sink.cuh): BC6H blocks -> BT.2020 PQ P010 planes, frame f's at luma / chroma + f*frame_stride.
+// Signedness per frame from frame_formats, or is_signed for all.  Launches count as bc_decode.
+uint32_t launch_bc6h_decode_yuv_pq(const uint8_t *blocks, uint32_t frames, uint64_t blocks_stride, uint32_t width, uint32_t height,
+                                   uint8_t *luma, uint8_t *chroma, uint64_t frame_stride, uint64_t pitch, unsigned color_space,
+                                   unsigned unit_nits, cudaStream_t st, const uint32_t *frame_results, const uint32_t *frame_formats,
+                                   bool is_signed)
+{
+    const uint16_t *table = pq_table(unit_nits, kPqOut);
+    if (!table) return HapResult_Internal_Error;
+    const YuvOutGeom g = yuv_out_geom(width, height, (uint32_t)pitch, blocks_stride, frame_stride, yuv_pq_out_coeffs(color_space));   // (pitch < 2^32)
+    for (uint32_t f0 = 0; f0 < frames; f0 += kBcFramesPerLaunch) {
+        const dim3 grid((unsigned)yuv_out_ctas(g), frames - f0 < kBcFramesPerLaunch ? frames - f0 : kBcFramesPerLaunch);
+        HAP_KLAUNCH(kStBcDecode, bc6h_decode_yuv_kernel, grid, dim3(kBcThreads), 0, st, blocks + f0 * g.in_stride, g, luma + f0 * g.frame_bytes,
+                    chroma + f0 * g.frame_bytes, frame_results ? frame_results + f0 : nullptr, frame_formats ? frame_formats + f0 : nullptr,
+                    is_signed ? 1u : 0u, table);
     }
     return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
 }
@@ -791,8 +815,8 @@ __global__ void ring_wait_kernel(const unsigned int *flag, unsigned int value, u
 }
 }  // namespace
 
-// The single-frame picture decoders (HapB200DecodeRGBA, HapB200DecodeRGBAHalf, HapB200DecodeYUV): textures 0 .. count-1 of
-// the frame, t[i] bytes each, are decoded by HapDecode into device scratch (a texture that does not fill its room: Bad_Frame);
+// The single-frame picture decoders (HapB200DecodeRGBA, HapB200DecodeRGBAHalf, HapB200DecodeYUV, HapB200DecodeYUVPQ): textures
+// 0 .. count-1 of the frame, t[i] bytes each, are decoded by HapDecode into device scratch (a texture that does not fill its room: Bad_Frame);
 // then launch(textures, picture, tight row bytes, stream) writes a tight picture of bpp bytes per pixel, which is copied to the
 // caller's rows.  With a `chroma` plane the picture has a second plane of height/2 rows of the same width, which launch writes
 // at picture + tight * height and which is copied to chroma's rows (rowBytes apart, as the first plane's).
@@ -1718,6 +1742,32 @@ unsigned int HapB200BlockDecodeHalfBatch(const void *blocks, unsigned int frames
     });
 }
 
+// the bytes of the one BC6H texture of a width x height Hap HDR frame
+static uint64_t bc6h_texture_bytes(unsigned width, unsigned height) { return (uint64_t)(width / 4) * (height / 4) * 16; }
+
+// The texture half of the Hap HDR batch decoders (HapB200DecodeRGBAHalfBatch, HapB200DecodeYUVPQBatch): texture 0 of every
+// frame decoded into device scratch `tex` (frame f at f * align16(bc6h_texture_bytes)) and its format into `formats`, both
+// allocated here, and results[f] set as HapB200DecodeRGBAHalfBatch reports it.
+static uint32_t decode_bc6h_textures_batch(const void *in, unsigned frames, unsigned long inStride, const unsigned long long *inBytes,
+                                           unsigned maxChunks, unsigned width, unsigned height, DevBuf &tex, DevBuf &formats,
+                                           unsigned *results, cudaStream_t st)
+{
+    const uint64_t t0 = bc6h_texture_bytes(width, height), stride = align16(t0);
+    DevBuf used(st);
+    if (!tex.alloc(stride * frames + 16) || !used.alloc(8ull * frames) || !formats.alloc(4ull * frames)) {
+        cudaGetLastError();
+        return HapResult_Internal_Error;
+    }
+    // texture 0 of every frame, offered exactly its BC6H size; then a frame that is not one BC6H texture of that size
+    // reports Bad_Frame, other failures keep the decoder's code, and failed frames are zeroed
+    const uint32_t r = launch_decode_batch((const uint8_t *)in, frames, inStride, inBytes, 0, maxChunks, tex.as<uint8_t>(), stride, t0,
+                                           used.as<unsigned long long>(), formats.as<uint32_t>(), results, st);
+    if (r != HapResult_No_Error) return r;
+    HAP_KLAUNCH(kStCollect, hap_check_bc6h_frames_kernel, dim3((frames + 127) / 128), dim3(128), 0, st, (const uint8_t *)in, (uint64_t)inStride,
+                inBytes, frames, used.as<unsigned long long>(), formats.as<uint32_t>(), (unsigned long long)t0, results);
+    return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
+}
+
 unsigned int HapB200DecodeRGBAHalfBatch(const void *in, unsigned int frames, unsigned long inStride, const unsigned long long *inBytes,
                                         unsigned int maxChunks, unsigned int width, unsigned int height, void *rgbaHalf,
                                         unsigned long frameStride, unsigned long rowBytes, unsigned int *results, void *stream)
@@ -1726,43 +1776,46 @@ unsigned int HapB200DecodeRGBAHalfBatch(const void *in, unsigned int frames, uns
         return HapResult_Bad_Arguments;
     HAP_ENTER(in, rgbaHalf);
     return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
-        const uint64_t t0 = (uint64_t)(width / 4) * (height / 4) * 16, stride = align16(t0);
-        DevBuf tex(st), used(st), formats(st);
-        if (!tex.alloc(stride * frames + 16) || !used.alloc(8ull * frames) || !formats.alloc(4ull * frames)) {
-            cudaGetLastError();
-            return HapResult_Internal_Error;
-        }
-        // texture 0 of every frame, offered exactly its BC6H size; then a frame that is not one BC6H texture of that size
-        // reports Bad_Frame, other failures keep the decoder's code, and failed frames are zeroed
-        const uint32_t r = launch_decode_batch((const uint8_t *)in, frames, inStride, inBytes, 0, maxChunks, tex.as<uint8_t>(), stride, t0,
-                                               used.as<unsigned long long>(), formats.as<uint32_t>(), results, st);
+        DevBuf tex(st), formats(st);
+        const uint32_t r = decode_bc6h_textures_batch(in, frames, inStride, inBytes, maxChunks, width, height, tex, formats, results, st);
         if (r != HapResult_No_Error) return r;
-        HAP_KLAUNCH(kStCollect, hap_check_bc6h_frames_kernel, dim3((frames + 127) / 128), dim3(128), 0, st, (const uint8_t *)in, (uint64_t)inStride,
-                    inBytes, frames, used.as<unsigned long long>(), formats.as<uint32_t>(), (unsigned long long)t0, results);
-        return launch_bc6h_decode(tex.as<uint8_t>(), frames, stride, width, height, (uint8_t *)rgbaHalf, frameStride, rowBytes, st, results,
-                                  formats.as<uint32_t>(), false);
+        return launch_bc6h_decode(tex.as<uint8_t>(), frames, align16(bc6h_texture_bytes(width, height)), width, height, (uint8_t *)rgbaHalf,
+                                  frameStride, rowBytes, st, results, formats.as<uint32_t>(), false);
     });
 }
 
-unsigned int HapB200DecodeRGBAHalf(const void *inputBuffer, unsigned long inputBufferBytes, unsigned int width, unsigned int height,
-                                   void *rgbaHalf, unsigned long rowBytes)
+extern "C++" {
+// The single-frame Hap HDR decoders (HapB200DecodeRGBAHalf, HapB200DecodeYUVPQ): a frame that is not one BC6H texture of the
+// picture's size is Bad_Frame; else decode_frame_to_picture, with launch(texture, picture, tight, stream, is_signed).
+template <class Launch>
+static uint32_t decode_bc6h_frame_to_picture(const void *inputBuffer, unsigned long inputBufferBytes, unsigned width, unsigned height,
+                                             uint64_t bpp, void *picture, unsigned long rowBytes, Launch &&launch, void *chroma = nullptr)
 {
-    if (!inputBuffer || !rgba_geometry_ok(rgbaHalf, width, height, rowBytes, 0, false, 8)) return HapResult_Bad_Arguments;
     unsigned count = 0, fmt = 0;
     uint32_t r = HapGetFrameTextureCount(inputBuffer, inputBufferBytes, &count);
     if (r != HapResult_No_Error) return r;
     r = HapGetFrameTextureFormat(inputBuffer, inputBufferBytes, 0, &fmt);
     if (r != HapResult_No_Error) return r;
     if (count != 1 || !is_bc6h_format(fmt)) return HapResult_Bad_Frame;
-    const uint64_t t[2] = {(uint64_t)(width / 4) * (height / 4) * 16, 0};
-    r = decode_frame_to_picture(inputBuffer, inputBufferBytes, 1, t, width, height, 8, rgbaHalf, rowBytes,
-                                [&](const uint8_t *tex, uint8_t *img, uint64_t tight, cudaStream_t st) {
-                                    return launch_bc6h_decode(tex, 1, 0, width, height, img, 0, tight, st, nullptr, nullptr,
-                                                              fmt == HapFmt_RGB_BPTC_SFLOAT);
-                                });
+    const uint64_t t[2] = {bc6h_texture_bytes(width, height), 0};
+    r = decode_frame_to_picture(
+        inputBuffer, inputBufferBytes, 1, t, width, height, bpp, picture, rowBytes,
+        [&](const uint8_t *tex, uint8_t *img, uint64_t tight, cudaStream_t st) { return launch(tex, img, tight, st, fmt == HapFmt_RGB_BPTC_SFLOAT); },
+        chroma);
     // the room offered is the picture's texture size: a texture too large for it (HapDecode: Buffer_Too_Small) is not this
     // picture's texture either
     return r == HapResult_Buffer_Too_Small ? (uint32_t)HapResult_Bad_Frame : r;
+}
+}  // extern "C++"
+
+unsigned int HapB200DecodeRGBAHalf(const void *inputBuffer, unsigned long inputBufferBytes, unsigned int width, unsigned int height,
+                                   void *rgbaHalf, unsigned long rowBytes)
+{
+    if (!inputBuffer || !rgba_geometry_ok(rgbaHalf, width, height, rowBytes, 0, false, 8)) return HapResult_Bad_Arguments;
+    return decode_bc6h_frame_to_picture(inputBuffer, inputBufferBytes, width, height, 8, rgbaHalf, rowBytes,
+                                        [&](const uint8_t *tex, uint8_t *img, uint64_t tight, cudaStream_t st, bool sgn) {
+                                            return launch_bc6h_decode(tex, 1, 0, width, height, img, 0, tight, st, nullptr, nullptr, sgn);
+                                        });
 }
 
 // ---- Hap HDR encoding: RGBA16F -> BC6H (bc6h_encode.cuh) ----
@@ -1891,6 +1944,55 @@ unsigned int HapB200BlockEncodeYUVPQBatch(const void *luma, const void *chroma, 
     if (!yuv_pq_args_ok(colorSpace, unitNits)) return HapResult_Bad_Arguments;
     return block_encode_bc6h_batch(yuv_pq_picture(luma, chroma, colorSpace, unitNits), frames, frameStride, width, height, pitch,
                                    textureFormat, blocks, blocksStride, stream);
+}
+
+// ---- Hap HDR -> HDR10: BC6H -> P010, BT.2020, PQ, K8 with the HDR10 sink (yuv_sink.cuh) ----
+
+unsigned int HapB200BlockDecodeYUVPQBatch(const void *blocks, unsigned int frames, unsigned long blocksStride, unsigned int width,
+                                          unsigned int height, unsigned int textureFormat, void *luma, void *chroma, unsigned long frameStride,
+                                          unsigned long pitch, unsigned int colorSpace, unsigned int unitNits, void *stream)
+{
+    if (!blocks || frames == 0 || !is_bc6h_format(textureFormat) || !yuv_pq_args_ok(colorSpace, unitNits) ||
+        !yuv_geometry_ok(luma, chroma, width, height, pitch, frameStride, true, 2) || ((uintptr_t)blocks | blocksStride) % 16)
+        return HapResult_Bad_Arguments;
+    HAP_ENTER(blocks, luma);
+    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
+        return launch_bc6h_decode_yuv_pq((const uint8_t *)blocks, frames, blocksStride, width, height, (uint8_t *)luma, (uint8_t *)chroma,
+                                         frameStride, pitch, colorSpace, unitNits, st, nullptr, nullptr,
+                                         textureFormat == HapFmt_RGB_BPTC_SFLOAT);
+    });
+}
+
+unsigned int HapB200DecodeYUVPQBatch(const void *in, unsigned int frames, unsigned long inStride, const unsigned long long *inBytes,
+                                     unsigned int maxChunks, unsigned int width, unsigned int height, void *luma, void *chroma,
+                                     unsigned long frameStride, unsigned long pitch, unsigned int colorSpace, unsigned int unitNits,
+                                     unsigned int *results, void *stream)
+{
+    if (!in || !inBytes || !results || frames == 0 || maxChunks == 0 || !yuv_pq_args_ok(colorSpace, unitNits) ||
+        !yuv_geometry_ok(luma, chroma, width, height, pitch, frameStride, true, 2))
+        return HapResult_Bad_Arguments;
+    HAP_ENTER(in, luma);
+    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
+        DevBuf tex(st), formats(st);
+        const uint32_t r = decode_bc6h_textures_batch(in, frames, inStride, inBytes, maxChunks, width, height, tex, formats, results, st);
+        if (r != HapResult_No_Error) return r;
+        return launch_bc6h_decode_yuv_pq(tex.as<uint8_t>(), frames, align16(bc6h_texture_bytes(width, height)), width, height, (uint8_t *)luma,
+                                         (uint8_t *)chroma, frameStride, pitch, colorSpace, unitNits, st, results, formats.as<uint32_t>(), false);
+    });
+}
+
+unsigned int HapB200DecodeYUVPQ(const void *inputBuffer, unsigned long inputBufferBytes, unsigned int width, unsigned int height, void *luma,
+                                void *chroma, unsigned long pitch, unsigned int colorSpace, unsigned int unitNits)
+{
+    if (!inputBuffer || !yuv_pq_args_ok(colorSpace, unitNits) || !yuv_geometry_ok(luma, chroma, width, height, pitch, 0, false, 2))
+        return HapResult_Bad_Arguments;
+    return decode_bc6h_frame_to_picture(
+        inputBuffer, inputBufferBytes, width, height, 2, luma, pitch,
+        [&](const uint8_t *tex, uint8_t *img, uint64_t tight, cudaStream_t st, bool sgn) {
+            return launch_bc6h_decode_yuv_pq(tex, 1, 0, width, height, img, img + tight * height, 0, tight, colorSpace, unitNits, st, nullptr,
+                                             nullptr, sgn);
+        },
+        chroma);
 }
 
 // ---- include/hap_mov.h: QuickTime sample tables around Hap frames (host code only) -------------------------

@@ -14,7 +14,8 @@ HapB200Codec_Hap1, HapB200Codec_Hap5, HapB200Codec_HapY, HapB200Codec_HapM, HapB
 # BC7 encoders (encode_rgba_bc7, encode_rgba_bc7_batch, block_encode_bc7_batch) ask for it by name
 HapB200YUV_NV12, HapB200YUV_P010 = range(2)
 HapB200YUV_BT601_Limited, HapB200YUV_BT601_Full, HapB200YUV_BT709_Limited, HapB200YUV_BT709_Full = range(4)
-# BT.2020: taken only by the HDR10 encoders (encode_yuv_pq, encode_yuv_pq_batch, block_encode_yuv_pq_batch)
+# BT.2020: taken only by the HDR10 encoders (encode_yuv_pq, encode_yuv_pq_batch, block_encode_yuv_pq_batch) and decoders
+# (decode_yuv_pq, decode_yuv_pq_batch, block_decode_yuv_pq_batch)
 HapB200YUV_BT2020_Limited, HapB200YUV_BT2020_Full = 4, 5
 
 
@@ -98,6 +99,12 @@ class HapB200(HapABI):
         L.HapB200EncodeYUVPQBatch.argtypes = [vp, vp, u, ul, u, u, ul, u, u, u, u, u, vp, ul, vp, vp]
         L.HapB200BlockEncodeYUVPQBatch.restype = u
         L.HapB200BlockEncodeYUVPQBatch.argtypes = [vp, vp, u, ul, u, u, ul, u, u, u, vp, ul, vp]
+        L.HapB200DecodeYUVPQ.restype = u
+        L.HapB200DecodeYUVPQ.argtypes = [vp, ul, u, u, vp, vp, ul, u, u]
+        L.HapB200DecodeYUVPQBatch.restype = u
+        L.HapB200DecodeYUVPQBatch.argtypes = [vp, u, ul, vp, u, u, u, vp, vp, ul, ul, u, u, vp, vp]
+        L.HapB200BlockDecodeYUVPQBatch.restype = u
+        L.HapB200BlockDecodeYUVPQBatch.argtypes = [vp, u, ul, u, u, u, vp, vp, ul, ul, u, u, vp]
         for name, args in (("RingCreate", [C.c_int, ul, C.POINTER(vp), vp]), ("RingDestroy", [C.c_int, vp]),
                            ("RingOpen", [C.c_int, vp, C.POINTER(vp)]), ("RingClose", [C.c_int, vp]),
                            ("RingAttach", [C.c_int, C.c_int]), ("RingPublish", [C.c_int, vp, u, vp]), ("RingWait", [C.c_int, vp, u, u, vp])):
@@ -380,6 +387,34 @@ class HapB200(HapABI):
                                   blocks_stride, stream=None):
         return int(self.lib.HapB200BlockEncodeYUVPQBatch(luma, chroma, frames, frame_stride, w, h, pitch, color_space, unit_nits,
                                                          texture_format, blocks, blocks_stride, stream))
+
+    # -- Hap HDR (BC6H) -> HDR10 P010 (BT.2020, PQ): color_space HapB200YUV_BT2020_*, unit_nits the cd/m2 of 1.0 (1-10000);
+    #    planes as for decode_yuv with HapB200YUV_P010 (pitch default 2 * width)
+    def decode_yuv_pq(self, frame, w, h, color_space, unit_nits, pitch=None, luma=None, chroma=None, frame_bytes=None):
+        """frame, luma, chroma: buffer objects or (addr, nbytes).  Returns (result, (luma bytes, chroma bytes)) when it
+        allocates the planes (luma and chroma not given), else (result, None)."""
+        from .abi import _as_ptr
+        faddr, fn = _as_ptr(frame)
+        if frame_bytes is not None:
+            fn = frame_bytes
+        pitch = pitch or 2 * w
+        own = luma is None and chroma is None
+        if own:
+            luma, chroma = bytearray(pitch * h), bytearray(pitch * (h // 2))
+        laddr, _ = _as_ptr(luma)
+        caddr, _ = _as_ptr(chroma)
+        r = self.lib.HapB200DecodeYUVPQ(faddr, fn, w, h, laddr, caddr, pitch, color_space, unit_nits)
+        return int(r), ((bytes(luma), bytes(chroma)) if own and r == 0 else None)
+
+    def decode_yuv_pq_batch(self, frames_ptr, frames, in_stride, in_bytes, max_chunks, w, h, luma, chroma, frame_stride, pitch, color_space,
+                            unit_nits, results, stream=None):
+        return int(self.lib.HapB200DecodeYUVPQBatch(frames_ptr, frames, in_stride, in_bytes, max_chunks, w, h, luma, chroma, frame_stride,
+                                                    pitch, color_space, unit_nits, results, stream))
+
+    def block_decode_yuv_pq_batch(self, blocks, frames, blocks_stride, w, h, texture_format, luma, chroma, frame_stride, pitch,
+                                  color_space, unit_nits, stream=None):
+        return int(self.lib.HapB200BlockDecodeYUVPQBatch(blocks, frames, blocks_stride, w, h, texture_format, luma, chroma, frame_stride,
+                                                         pitch, color_space, unit_nits, stream))
 
     # -- delivery rings (include/hap_b200.h): frames written straight into another GPU's memory -----------------
     RING_HANDLE_BYTES = 64

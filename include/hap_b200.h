@@ -444,6 +444,68 @@ unsigned int HapB200BlockEncodeYUVPQBatch(const void *luma, const void *chroma, 
                                           unsigned long pitch, unsigned int colorSpace, unsigned int unitNits,
                                           unsigned int textureFormat, void *blocks, unsigned long blocksStride, void *stream);
 
+/* ---- Hap HDR (BC6H, "HapH") -> HDR10 P010 (BT.2020, SMPTE ST 2084 / PQ) --------------------------------------------------
+ * The decoders write the P010 pictures a video encoder takes for HEVC Main10 HDR10 (NVENC surfaces): the inverse of the HDR10
+ * encoders above.  The conversion is fused into the BC6H block decoder, so no RGBA16F picture is ever written.  The planes are
+ * exactly the conversion below applied to the RGBA16F picture that HapB200DecodeRGBAHalf / HapB200DecodeRGBAHalfBatch /
+ * HapB200BlockDecodeHalfBatch give for the same input; alpha is ignored.
+ * Planes, pitch, geometry, alignment and bytes written: those of HapB200DecodeYUV* with HapB200YUV_P010 (little-endian 16-bit
+ * words holding sample << 6; only the 2 * width bytes of each of the height luma rows and height/2 chroma rows are written:
+ * pitch slack and whatever lies between planes and frames stays as it was).  HDR10 is always 10-bit, so there is no layout
+ * argument.  colorSpace: HapB200YUV_BT2020_Limited or HapB200YUV_BT2020_Full.  unitNits: as for the HDR10 encoders, the
+ * luminance in cd/m2 that the value 1.0 stands for, 1 to 10000.  textureFormat (HapB200BlockDecodeYUVPQBatch): UF16 or SF16.
+ * Any other value, and any bad geometry, is refused with HapResult_Bad_Arguments before anything touches the GPU.  The first
+ * call with a unitNits on a device builds its table (62 KiB) on the host and uploads it, waiting for the copy; later calls
+ * reuse it.
+ * Results: HapB200DecodeYUVPQ answers exactly as HapB200DecodeRGBAHalf does (a frame that is not one BC6H texture of
+ * (width/4)*(height/4)*16 bytes: HapResult_Bad_Frame); HapB200DecodeYUVPQBatch reports in results[f] exactly what
+ * HapB200DecodeRGBAHalfBatch reports.  Each frame decodes as its own texture format says (UF16 or SF16).  A failed frame's
+ * RGBA16F picture is all zero, so its planes are black: Y = yOff, Cb = Cr = 512.
+ * The conversion, exactly:
+ *   1. Transfer, the inverse of the encoders' step 3: each of R, G and B, a binary16 h, becomes the 12-bit code P[h], where
+ *        P[h] = floor(4095 * OETF(min(value(h) * unitNits / 10000, 1)) + 1/2),
+ *        OETF(Y) = ((c1 + c2 * Y^m1) / (1 + c3 * Y^m1))^m2
+ *      with the ST 2084 constants of the encoders, for every non-negative finite h (0x0000 .. 0x7BFF).  A value whose sign
+ *      bit is set (SF16 negatives and -0) gives code 0.  P[0] = 0, every value at or above 10000 / unitNits gives 4095, and
+ *      P never decreases.  The block decoder writes no Inf or NaN.
+ *   2. Matrix, 12-bit R'G'B' to BT.2020 Y'CbCr (non-constant luminance): the rule of HAPB200_YUV_OUT_COEFFICIENTS with 4095
+ *      for 255 (L = 65536 * lumaScale / 4095, S = 65536 * chromaScale / 4095; Kr = 0.2627, Kb = 0.0593; limited range luma
+ *      offset 64, luma scale 876, chroma scale 896; full range offset 0, both scales 1023; chroma offset 512), which gives
+ *      the rows of HAPB200_YUV_PQ_OUT_COEFFICIENTS below; the derived entries make greys exactly neutral.  Then, as for
+ *      HapB200DecodeYUV with the codes for R, G and B:
+ *        Y = ((yR*R + yG*G + yB*B + 32768) >> 16) + yOff, clamped to 0..1023;
+ *        chroma at the default siting, Rs, Gs, Bs the [1 2 1] x [1 1] sums of the codes (column -1 clamped to 0),
+ *        Cb = ((cbR*Rs + cbG*Gs + cbB*Bs + 2^18) >> 19) + cOff,  Cr = ((crR*Rs + crG*Gs + crB*Bs + 2^18) >> 19) + cOff,
+ *      the shift arithmetic, each clamped to 0..1023.  Every intermediate is below 2^29.  Codes 4095 and 0 land on the
+ *      nominal white and black (Y = 940 / 64 limited, 1023 / 0 full).  12 bits are four times the output's resolution, so
+ *      the matrix adds at most about 0.1 of a code before its final rounding.
+ * Round trip: a flat P010 colour converted to R'G'B' by HAPB200_YUV_PQ_COEFFICIENTS and back by the rows below returns
+ * exactly wherever its R'G'B' is not clamped, and P[T[c]] = c for every code c at unitNits up to 123 (above, only the lowest
+ * codes, whose halves cannot tell neighbours apart, miss: c = 1 at 203; some codes below 16 at 1000, below 180 at 10000).  So a flat HDR10
+ * picture encoded by HapB200EncodeYUVPQ and decoded here at the same colorSpace and unitNits comes back byte for byte
+ * within those bounds. */
+/* row colorSpace - HapB200YUV_BT2020_Limited: {yR, yG, yB, cbR, cbG, cbB, crR, crG, crB, yOff, cOff} */
+#define HAPB200_YUV_PQ_OUT_COEFFICIENTS                                                                                    \
+    {                                                                                                                      \
+        {3683, 9505, 831, -2002, -5168, 7170, 7170, -6593, -577, 64, 512},  /* P010 BT.2020 limited */                     \
+        {4301, 11100, 971, -2286, -5900, 8186, 8186, -7528, -658, 0, 512}   /* P010 BT.2020 full    */                     \
+    }
+
+/* one Hap HDR frame (host or device pointers, any alignment, any pitch) -> one HDR10 P010 picture */
+unsigned int HapB200DecodeYUVPQ(const void *inputBuffer, unsigned long inputBufferBytes, unsigned int width, unsigned int height,
+                                void *luma, void *chroma, unsigned long pitch, unsigned int colorSpace, unsigned int unitNits);
+/* frames x Hap HDR frame (device, as HapB200DecodeRGBAHalfBatch) -> frames x picture (device): frame f's planes at
+ * luma + f*frameStride, chroma + f*frameStride */
+unsigned int HapB200DecodeYUVPQBatch(const void *in, unsigned int frames, unsigned long inStride, const unsigned long long *inBytes,
+                                     unsigned int maxChunks, unsigned int width, unsigned int height, void *luma, void *chroma,
+                                     unsigned long frameStride, unsigned long pitch, unsigned int colorSpace, unsigned int unitNits,
+                                     unsigned int *results, void *stream);
+/* bare BC6H textures (device, textureFormat UF16 or SF16, as HapB200BlockDecodeHalfBatch) -> pictures */
+unsigned int HapB200BlockDecodeYUVPQBatch(const void *blocks, unsigned int frames, unsigned long blocksStride, unsigned int width,
+                                          unsigned int height, unsigned int textureFormat, void *luma, void *chroma,
+                                          unsigned long frameStride, unsigned long pitch, unsigned int colorSpace,
+                                          unsigned int unitNits, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

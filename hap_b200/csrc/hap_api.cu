@@ -93,6 +93,7 @@ struct DeviceState {
     int k5_ctas_per_sm = 1;   // resident CTAs of the fragment compressor per SM (its persistent grid is this x sm_count)
     int fused_ctas_per_sm = 1;   // the same for the fused Hap Q encoder (hapq_fused.cuh)
     int fused_place_ctas_per_sm = 1;   // ... and for its variant that writes the frames itself
+    int units_ctas_per_sm = 1;   // ... and for the Snappy decoder's unit kernel (snappy_execute_units_kernel)
 };
 DeviceState g_dev[kMaxDevices];
 std::atomic<int> g_default_device{-1};
@@ -121,7 +122,13 @@ void device_init(int dev)
     ok = ok && cudaFuncSetAttribute(hapq_fused_place_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(EncodeSmem)) == cudaSuccess;
     ok = ok && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&d.fused_place_ctas_per_sm, hapq_fused_place_kernel, kEncThreads,
                                                              sizeof(EncodeSmem)) == cudaSuccess;
+#if HAPB200_EX_UNIT_KERNEL
+    ok = ok && cudaFuncSetAttribute(snappy_execute_units_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(UnitSmem)) == cudaSuccess;
+    ok = ok && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&d.units_ctas_per_sm, snappy_execute_units_kernel, kUxThreads,
+                                                             sizeof(UnitSmem)) == cudaSuccess;
+#endif
     if (!ok) { cudaGetLastError(); return; }
+    if (d.units_ctas_per_sm < 1) d.units_ctas_per_sm = 1;
     if (d.fused_place_ctas_per_sm < 1) d.fused_place_ctas_per_sm = 1;
     if (d.k5_ctas_per_sm < 1) d.k5_ctas_per_sm = 1;
     if (d.fused_ctas_per_sm < 1) d.fused_ctas_per_sm = 1;
@@ -182,6 +189,9 @@ struct DeviceGuard {
     if (!hap_device_guard_.ok) return HapResult_Internal_Error
 
 inline int sm_count() { return g_dev[t_device].sm_count; }
+#if HAPB200_EX_UNIT_KERNEL
+inline int units_ctas_per_sm() { return g_dev[t_device].units_ctas_per_sm; }
+#endif
 const cudaStream_t kLegacyStream = cudaStreamLegacy;
 // NULL-stream calls and the host-pointer entry points that touch caller-owned device buffers run on the LEGACY default
 // stream: it orders itself against every blocking stream of the process, so buffers a caller produced on its own (blocking)
@@ -687,6 +697,12 @@ struct DecodePasses {
                     wins.as<DecWin>(), win_cap, c);
         HAP_KLAUNCH(kStSnappyIndex, snappy_index_kernel, dim3(njobs), dim3(kIdxThreads), sizeof(IndexSmem), st, jobs, (int)njobs, 0u,
                     wins.as<DecWin>(), win_cap, entries.as<uint8_t>(), entry_slots, c);
+#if HAPB200_EX_UNIT_KERNEL
+        // the fragments of embedded indexes first (without the index there are none); the execute kernel takes the rest
+        if (g_use_index.load())
+            HAP_KLAUNCH(kStSnappyDecode, snappy_execute_units_kernel, dim3((unsigned)sm_count() * (unsigned)units_ctas_per_sm()), dim3(kUxThreads),
+                        sizeof(UnitSmem), st, jobs, njobs, wins.as<DecWin>(), c, done.as<uint32_t>());
+#endif
         HAP_KLAUNCH(kStSnappyDecode, snappy_execute_kernel, dim3(ex_grid), dim3(kExThreads), sizeof(ExecSmem), st, jobs, njobs, 0u, wins.as<DecWin>(), c,
                     done.as<uint32_t>());
         return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
@@ -1012,6 +1028,22 @@ int HapB200StageTimes(double *ms, unsigned long long *launches, int n)
     cudaGetLastError();
     return kStCount;
 }
+
+#if HAPB200_EX_PHASE_CLOCKS
+// Measurement builds only (-DHAPB200_EX_PHASE_CLOCKS=1): the unit path's clocks per phase summed over every CTA of the
+// current device since the last call, then the unit windows and the pointer-jumping rounds (snappy_decode.cuh, kPh*).
+// Synchronises the device and resets the sums.  Returns the number of slots.
+int HapB200UnitPhaseClocks(unsigned long long *out, int n)
+{
+    cudaDeviceSynchronize();
+    unsigned long long v[kPhSlots] = {};
+    if (cudaMemcpyFromSymbol(v, g_ex_phase_clocks, sizeof v) != cudaSuccess) { cudaGetLastError(); return -1; }
+    const unsigned long long zero[kPhSlots] = {};
+    cudaMemcpyToSymbol(g_ex_phase_clocks, zero, sizeof zero);
+    for (int i = 0; i < n && i < kPhSlots; i++) out[i] = v[i];
+    return kPhSlots;
+}
+#endif
 
 // hap.c:324-353
 unsigned long HapMaxEncodedLength(unsigned int count, unsigned long *lengths, unsigned int *textureFormats,

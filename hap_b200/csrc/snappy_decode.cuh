@@ -27,6 +27,8 @@
 //       source bytes are not final yet wait for a later round; windows of an on-the-fly index wait (one acquire) for
 //       the earlier windows their copies reach into.  Fragments of an embedded index made of 8-byte elements (this
 //       encoder's) skip the descriptors and tiles: they are decoded as 4096 eight-byte units (execute_units).
+//   snappy_execute_units_kernel runs before it and decodes those fragments in a kernel of their own that keeps more
+//       windows resident per SM; the execute kernel then takes only the windows it left.
 // Every decision is taken on device; the host reads one status word per chunk.
 #pragma once
 #include "block_primitives.cuh"
@@ -71,7 +73,12 @@ struct DecodeCtl {
     uint32_t overflow;         // a chunk did not fit the list (cannot happen with the host's sizing; checked)
     uint32_t ticket[2];        // per execute pass: next ticket.  Ticket T = window (T / njobs) of chunk (T % njobs): the
     uint32_t max_k[2];         //   k-th windows of ALL chunks come before any (k+1)-th, so that a window rarely has to wait for
-    uint32_t pad[1];           //   its predecessor and 444 resident CTAs work on 444 different chunks.  max_k: most windows any chunk has.
+                               //   its predecessor and 444 resident CTAs work on 444 different chunks.  max_k: most windows any chunk has.
+    uint32_t unit_ticket;      // snappy_execute_units_kernel: next ticket (window k = T / njobs of chunk T % njobs, k < max_k_units)
+    uint32_t max_k_units;      //   most windows any chunk with an embedded index has
+    uint32_t units_ran;        // nonzero once that kernel ran: pass 0 of the execute kernel then draws max_k_rest * njobs tickets and
+    uint32_t max_k_rest;       //   skips the windows it finished (done[w] != 0).  max_k_rest: (k + 1) of the last pass-0 window that
+                               //   is not an embedded-index fragment, or that the unit kernel left undone
 };
 
 constexpr uint32_t kSrcIn = 0u << 30, kSrcOut = 1u << 30, kSrcRun = 2u << 30, kSrcMask = 3u << 30, kPosMask = (1u << 30) - 1;
@@ -374,6 +381,7 @@ __global__ void __launch_bounds__(kIdxThreads, 4) snappy_index_kernel(ChunkJob *
         job.win_base = base;
         job.win_count = emitted;
         atomicMax(&ctl->max_k[pass], emitted);
+        if (pass == 0) atomicMax(&ctl->max_k_rest, emitted);
         job.mode = done_mode;
     }
 }
@@ -407,6 +415,7 @@ __global__ void hap_build_windows_kernel(ChunkJob *jobs, uint32_t njobs, uint32_
         if (base + cnt > win_cap || base + cnt < base) { job.status = HapResult_Internal_Error; atomicExch(&ctl->overflow, 1u); return; }
         job.win_base = base; job.win_count = cnt; job.mode = kJobReady;
         atomicMax(&ctl->max_k[0], cnt);
+        atomicMax(&ctl->max_k_rest, cnt);
         for (uint32_t i = 0; i < cnt; i++) {
             DecWin w;
             w.job = j; w.kind = kWinRaw; w.in_off = i * kRawWindow; w.in_len = n - i * kRawWindow < kRawWindow ? n - i * kRawWindow : kRawWindow;
@@ -440,6 +449,7 @@ __global__ void hap_build_windows_kernel(ChunkJob *jobs, uint32_t njobs, uint32_
     if (base + nf > win_cap || base + nf < base) { job.status = HapResult_Internal_Error; job.mode = kJobFinished; atomicExch(&ctl->overflow, 1u); return; }
     job.win_base = base; job.win_count = nf;
     atomicMax(&ctl->max_k[0], nf);
+    atomicMax(&ctl->max_k_units, nf);
     uint32_t in_off = pre;
     const uint8_t *ent = job.index + 2 * nf;
     for (uint32_t f = 0; f < nf; f++) {
@@ -494,6 +504,48 @@ constexpr int kFlattenHops = 12;
 #ifndef HAPB200_EX_UNIT_PATH
 #define HAPB200_EX_UNIT_PATH 1
 #endif
+// -DHAPB200_EX_PHASE_CLOCKS=1 (measurement builds only, tools/measure_unit_phases.py): thread 0 of every CTA adds up
+// clock64() per phase of the unit path in shared memory and folds its sums into g_ex_phase_clocks when the CTA ends.
+// Phases end at barriers where there is one, so a phase's clocks are those of the CTA, not of thread 0 alone.
+#ifndef HAPB200_EX_PHASE_CLOCKS
+#define HAPB200_EX_PHASE_CLOCKS 0
+#endif
+enum : int { kPhStage = 0, kPhWalk, kPhScan, kPhRecords, kPhMap, kPhRounds, kPhWrite, kPhOther, kPhCount };
+enum : int { kPhUnitWindows = kPhCount, kPhRoundCount, kPhSlots };   // counters kept behind the phase clocks
+#if HAPB200_EX_PHASE_CLOCKS && !defined(HAPB200_EMU)
+__device__ unsigned long long g_ex_phase_clocks[kPhSlots];
+__shared__ unsigned long long s_ex_phase[kPhSlots + 1];   // [kPhSlots]: clock of the last mark
+#define HAP_PHASE_BEGIN()                                                                 \
+    do {                                                                                  \
+        if (threadIdx.x == 0) {                                                           \
+            for (int q_ = 0; q_ < kPhSlots; q_++) s_ex_phase[q_] = 0;                     \
+            s_ex_phase[kPhSlots] = clock64();                                             \
+        }                                                                                 \
+    } while (0)
+#define HAP_PHASE_MARK(ph)                                                                \
+    do {                                                                                  \
+        if (threadIdx.x == 0) {                                                           \
+            const unsigned long long c_ = clock64();                                      \
+            s_ex_phase[ph] += c_ - s_ex_phase[kPhSlots];                                  \
+            s_ex_phase[kPhSlots] = c_;                                                    \
+        }                                                                                 \
+    } while (0)
+#define HAP_PHASE_COUNT(slot)                                                             \
+    do {                                                                                  \
+        if (threadIdx.x == 0) s_ex_phase[slot]++;                                         \
+    } while (0)
+#define HAP_PHASE_END()                                                                   \
+    do {                                                                                  \
+        if (threadIdx.x == 0)                                                             \
+            for (int q_ = 0; q_ < kPhSlots; q_++) atomicAdd(&g_ex_phase_clocks[q_], s_ex_phase[q_]); \
+    } while (0)
+#else
+#define HAP_PHASE_BEGIN() do {} while (0)
+#define HAP_PHASE_MARK(ph) do {} while (0)
+#define HAP_PHASE_COUNT(slot) do {} while (0)
+#define HAP_PHASE_END() do {} while (0)
+#endif
+
 constexpr uint32_t kExUnits = kIndexFragBytes / 8;   // 8-byte output units of a fragment (unit path)
 constexpr uint32_t kUnitLit = kExUnits;              // unit map value >= this: literal bytes at window byte (value - kUnitLit)
 constexpr int kUnitMaxRounds = 24;                   // pointer jumping over chains of <= 4096 units ends within 13 rounds
@@ -712,15 +764,20 @@ __device__ __forceinline__ WalkResult walk_piece(const uint8_t *cin, uint32_t wb
 // The next ticket that names an existing window (window k = T / njobs of chunk T % njobs) and that window's record, fetched
 // by thread 0 one window AHEAD, right after the current window's bulk copy has been issued: the atomic and the global
 // loads then overlap the copy instead of standing alone in front of a barrier.  (Not inlined: one thread's cold path.)
+// finished: the unit kernel's per-window flags (done[]) when it ran before this pass, else nullptr.
 __device__ __noinline__ void fetch_next_window(const ChunkJob *jobs, uint32_t njobs, uint32_t pass, uint32_t want_mode, unsigned long long n_tickets,
-                                               const DecWin *wins, DecodeCtl *ctl, DecWin *win_out, uint32_t *ticket_out)
+                                               const DecWin *wins, DecodeCtl *ctl, DecWin *win_out, uint32_t *ticket_out, const uint32_t *finished)
 {
     uint32_t w = 0xFFFFFFFFu;
     for (;;) {
         const unsigned long long T = atomicAdd(&ctl->ticket[pass], 1u);
         if (T >= n_tickets) break;
         const uint32_t k = (uint32_t)(T / njobs), j = (uint32_t)(T % njobs);
-        if (jobs[j].compressor != 0 && jobs[j].mode == want_mode && k < jobs[j].win_count) { w = jobs[j].win_base + k; break; }
+        if (jobs[j].compressor != 0 && jobs[j].mode == want_mode && k < jobs[j].win_count) {
+            w = jobs[j].win_base + k;
+            if (finished && finished[w] != 0) { w = 0xFFFFFFFFu; continue; }
+            break;
+        }
     }
     *ticket_out = w;
     if (w != 0xFFFFFFFFu) *win_out = wins[w];
@@ -773,6 +830,7 @@ __device__ __noinline__ bool execute_units(ExecSmem &S, int &crossing, uint32_t 
         }
     }
     __syncthreads();
+    HAP_PHASE_MARK(kPhRecords);
     if (crossing) return false;
     const uint32_t U = out_len >> 3, u0 = kUnitStripLen * (uint32_t)t;
     uint32_t r[kUnitStripLen];
@@ -803,6 +861,7 @@ __device__ __noinline__ bool execute_units(ExecSmem &S, int &crossing, uint32_t 
         map4[2 * t + h] = make_uint4((v[8 * h] & 0xFFFFu) | (v[8 * h + 1] << 16), (v[8 * h + 2] & 0xFFFFu) | (v[8 * h + 3] << 16),
                                      (v[8 * h + 4] & 0xFFFFu) | (v[8 * h + 5] << 16), (v[8 * h + 6] & 0xFFFFu) | (v[8 * h + 7] << 16));
     pending = __syncthreads_or(pending);
+    HAP_PHASE_MARK(kPhMap);
     for (int round = 0; pending; round++) {
         pending = 0;
         for (uint32_t u = t; u < U; u += kExThreads) {
@@ -814,6 +873,8 @@ __device__ __noinline__ bool execute_units(ExecSmem &S, int &crossing, uint32_t 
             }
         }
         pending = __syncthreads_or(pending);
+        HAP_PHASE_MARK(kPhRounds);
+        HAP_PHASE_COUNT(kPhRoundCount);
         if (pending && round == kUnitMaxRounds) return false;   // (cannot happen: chains are at most 4096 units deep)
     }
     // group g = destination bytes [16g - m, 16g - m + 16) of the fragment, m = misalignment of its first byte
@@ -858,7 +919,11 @@ __global__ void __launch_bounds__(kExThreads, HAPB200_EX_MIN_BLOCKS) snappy_exec
     HAP_DYN_SMEM(smem_raw);
     ExecSmem &S = *reinterpret_cast<ExecSmem *>(smem_raw);
     const int t = threadIdx.x;
-    const uint32_t max_k = ctl->max_k[pass];   // final: every kernel that lists windows ran before this one
+    // final: every kernel that lists windows ran before this one.  Behind the unit kernel, pass 0 takes only the chunks
+    // whose windows it did not all finish, and skips the windows it did.
+    const bool behind_units = pass == 0 && ctl->units_ran != 0;
+    const uint32_t max_k = behind_units ? ctl->max_k_rest : ctl->max_k[pass];
+    const uint32_t *finished = behind_units ? done : nullptr;
     const uint32_t want_mode = pass == 0 ? (uint32_t)kJobReady : (uint32_t)kJobRepaired;
     const unsigned long long n_tickets = (unsigned long long)max_k * njobs;
     if (t == 0) {
@@ -866,8 +931,9 @@ __global__ void __launch_bounds__(kExThreads, HAPB200_EX_MIN_BLOCKS) snappy_exec
         for (int q = 0; q < 2; q++) { S.flags[q].min_src = 0xFFFFFFFFu; S.flags[q].fail = 0; S.flags[q].fail_desc = 0; S.flags[q].mismatch = 0; }
     }
     uint32_t phase = 0;
+    HAP_PHASE_BEGIN();
     __syncthreads();
-    auto fetch_window = [&](uint32_t slot) { fetch_next_window(jobs, njobs, pass, want_mode, n_tickets, wins, ctl, &S.slot[slot & 1].win, &S.slot[slot & 1].ticket); };
+    auto fetch_window = [&](uint32_t slot) { fetch_next_window(jobs, njobs, pass, want_mode, n_tickets, wins, ctl, &S.slot[slot & 1].win, &S.slot[slot & 1].ticket, finished); };
     if (t == 0) fetch_window(0);
     for (uint32_t it = 0;; it++) {
         ExecSmem::Flags &F = S.flags[it & 1];
@@ -898,6 +964,7 @@ __global__ void __launch_bounds__(kExThreads, HAPB200_EX_MIN_BLOCKS) snappy_exec
                 for (uint32_t i = t; i < win.in_len; i += kExThreads) d[i] = s[i];
             }
             if (t == 0) fetch_window(it + 1);
+            HAP_PHASE_MARK(kPhOther);
             continue;   // nobody waits for a verbatim window
         }
         const bool embedded = win.first == kNoDeps;     // entries come from the frame: nothing in them is trusted
@@ -920,6 +987,7 @@ __global__ void __launch_bounds__(kExThreads, HAPB200_EX_MIN_BLOCKS) snappy_exec
         hap_mbar_wait(&S.bar, phase);
         phase ^= 1;
         __syncthreads();
+        HAP_PHASE_MARK(kPhStage);
         const uint32_t a_sh = (uint32_t)((uintptr_t)(src + win.in_off) & 15);
         const uint8_t *cin = S.cin + 32 + a_sh;
         const uint32_t wb = win.in_off;
@@ -946,6 +1014,7 @@ __global__ void __launch_bounds__(kExThreads, HAPB200_EX_MIN_BLOCKS) snappy_exec
             }
         }
         if (wr.invalid) F.fail = 1;
+        HAP_PHASE_MARK(kPhWalk);
         uint32_t total_e, total_o;
         const uint32_t ebase = block_excl_sum<kExThreads>(wr.count, &total_e, S.scratch);
         const uint32_t obase = block_excl_sum<kExThreads>(wr.out_bytes > 0x40000000u ? 0x40000000u : wr.out_bytes, &total_o, S.scratch);
@@ -967,6 +1036,7 @@ __global__ void __launch_bounds__(kExThreads, HAPB200_EX_MIN_BLOCKS) snappy_exec
 #else
         __syncthreads();
 #endif
+        HAP_PHASE_MARK(kPhScan);
         if (F.fail || F.mismatch) {
             if (t == 0) { job.status = embedded ? kStatusIndexMismatch : (uint32_t)HapResult_Bad_Frame; __threadfence(); hap_st_release(&done[w], 1u); }
             continue;
@@ -978,6 +1048,8 @@ __global__ void __launch_bounds__(kExThreads, HAPB200_EX_MIN_BLOCKS) snappy_exec
             int &crossing = F.fail_desc;
             const bool ok = execute_units(S, crossing, 32 + a_sh, wb, in_end, entered, my_lo + ent, my_hi, obase, dst + win.out_off, win.out_len);
             __syncthreads();
+            HAP_PHASE_MARK(kPhWrite);
+            HAP_PHASE_COUNT(kPhUnitWindows);
             if (t == 0) {
                 if (!ok) job.status = kStatusIndexMismatch;
 #ifdef HAPB200_EMU
@@ -1183,7 +1255,298 @@ __global__ void __launch_bounds__(kExThreads, HAPB200_EX_MIN_BLOCKS) snappy_exec
             __threadfence();
             hap_st_release(&done[w], 1u);
         }
+        HAP_PHASE_MARK(kPhOther);
     }
+    HAP_PHASE_END();
+}
+
+// =====================================================================================================================
+//  unit kernel: the unit path on its own, ahead of the execute kernel
+// =====================================================================================================================
+// snappy_execute_units_kernel decodes the pass-0 fragments of embedded indexes (win.first == kNoDeps) whose elements are
+// all 8-byte granular, with the decisions of the execute kernel's unit path (execute_units), in a kernel that holds only
+// what that path needs: the staged window and one 16-bit unit map built in place over the records, 41 KB of shared memory
+// against the execute kernel's 54 KB, so that 5 windows are resident per SM instead of 4.  Per window: one scan (output
+// bytes) instead of two, the element owning each unit found by one max-scan over packed (unit, record) keys, and the
+// period of an overlapping copy followed by a counter instead of a modulo per unit.  Fragments of an embedded index never
+// wait for each other, so windows are taken in list order.  A window it finishes (decoded, or found not to match its
+// index: kStatusIndexMismatch, the repair pass decodes the chunk) gets done[w] = 1; a window it declines (an element that
+// is not 8-byte granular) is left to the execute kernel, which then skips the finished ones (DecodeCtl::units_ran).
+#ifndef HAPB200_EX_UNIT_KERNEL
+#define HAPB200_EX_UNIT_KERNEL 1
+#endif
+#ifndef HAPB200_UX_MIN_BLOCKS
+#define HAPB200_UX_MIN_BLOCKS 5
+#endif
+constexpr int kUxThreads = 256;
+
+struct UnitSmem {
+    uint8_t cin[kExMaxIn + kExLook + 48];            // staged window, cin[a + i] = byte i of the window (a = its address & 15)
+    uint16_t map[kExUnits];                          // records, then (in place) the source of every 8-byte unit
+    uint8_t landed[kUxThreads];                      // a chain exit lands in this piece
+    uint32_t scratch[kUxThreads / 32];
+    DecWin win[2];                                   // the window being worked on and the next one (fetched by thread 0)
+    uint32_t ticket[2];
+    hap_mbar_t bar;
+    int mismatch[2];                                 // per window, two sets used alternately (as ExecSmem::flags)
+};
+
+#ifdef HAPB200_EMU
+inline uint64_t &emu_unit_kernel_windows() { static uint64_t n = 0; return n; }   // windows this kernel decoded (tests only)
+inline uint64_t &emu_unit_kernel_declined() { static uint64_t n = 0; return n; }  // windows it left to the execute kernel
+#endif
+
+// thread 0: the next window this kernel takes, and its record.  Only windows a chunk lists are looked at (the list has
+// reserved slots that were never written).
+__device__ __noinline__ void fetch_unit_window(const ChunkJob *jobs, uint32_t njobs, unsigned long long n_tickets, const DecWin *wins, DecodeCtl *ctl,
+                                               DecWin *win_out, uint32_t *ticket_out)
+{
+    uint32_t w = 0xFFFFFFFFu;
+    for (;;) {
+        const unsigned long long T = atomicAdd(&ctl->unit_ticket, 1u);
+        if (T >= n_tickets) break;
+        const uint32_t k = (uint32_t)(T / njobs), j = (uint32_t)(T % njobs);
+        if (jobs[j].compressor == 0 || jobs[j].mode != kJobReady || k >= jobs[j].win_count) continue;
+        const DecWin x = wins[jobs[j].win_base + k];
+        if (x.kind == kWinSnappy && x.first == kNoDeps) { *win_out = x; w = jobs[j].win_base + k; break; }
+    }
+    *ticket_out = w;
+}
+
+__global__ void __launch_bounds__(kUxThreads, HAPB200_UX_MIN_BLOCKS) snappy_execute_units_kernel(ChunkJob *jobs, uint32_t njobs, const DecWin *wins,
+                                                                                                DecodeCtl *ctl, uint32_t *done)
+{
+    static_assert(kExUnits == kUnitStripLen * kUxThreads, "16 units per thread");
+    HAP_DYN_SMEM(smem_raw);
+    UnitSmem &S = *reinterpret_cast<UnitSmem *>(smem_raw);
+    const int t = threadIdx.x;
+    const unsigned long long n_tickets = (unsigned long long)ctl->max_k_units * njobs;   // (final: the listing kernels ran before)
+    uint4 *map4 = reinterpret_cast<uint4 *>(S.map);
+    if (t == 0) {
+        hap_mbar_init(&S.bar, 1);
+        S.mismatch[0] = 0;
+        S.mismatch[1] = 0;
+        if (blockIdx.x == 0) ctl->units_ran = 1;   // (read by the execute kernel, which runs behind this one)
+        fetch_unit_window(jobs, njobs, n_tickets, wins, ctl, &S.win[0], &S.ticket[0]);
+    }
+    uint32_t phase = 0;
+    HAP_PHASE_BEGIN();
+    for (uint32_t it = 0;; it++) {
+        __syncthreads();   // the previous window's reads of the staging buffer and the map are over; slot it & 1 is filled
+        const uint32_t w = S.ticket[it & 1];
+        if (w == 0xFFFFFFFFu) break;
+        int &mismatch = S.mismatch[it & 1];
+        if (t == 0) S.mismatch[(it + 1) & 1] = 0;
+        const DecWin win = S.win[it & 1];
+        ChunkJob &job = jobs[win.job];
+        const uint8_t *__restrict__ src = job.src;
+        uint8_t *__restrict__ out = job.dst + win.out_off;
+        const uint32_t in_end = job.src_bytes, expected = job.dst_bytes;
+        const uint32_t sub = 1u << win.sub_log2;
+        const uint32_t nsub_all = (win.in_len + sub - 1) >> win.sub_log2;
+        const uint32_t nsub = nsub_all < (uint32_t)kUxThreads ? nsub_all : (uint32_t)kUxThreads;   // the last thread walks to the window's end
+        const bool fits = win.in_len <= (uint32_t)kExMaxIn && win.in_off <= in_end && win.in_len <= in_end - win.in_off &&
+                          win.out_off <= expected && win.out_len <= expected - win.out_off && win.out_len <= kIndexFragBytes;
+        if (!fits) {   // (uniform)
+            if (t == 0) {
+                job.status = kStatusIndexMismatch;
+                done[w] = 1u;
+                fetch_unit_window(jobs, njobs, n_tickets, wins, ctl, &S.win[(it + 1) & 1], &S.ticket[(it + 1) & 1]);
+            }
+            continue;
+        }
+        const uint32_t staged = in_end - win.in_off < win.in_len + (uint32_t)kExLook ? in_end - win.in_off : win.in_len + (uint32_t)kExLook;
+        stage_bytes(S.cin, src + win.in_off, staged, &S.bar, t);
+        if (t == 0) fetch_unit_window(jobs, njobs, n_tickets, wins, ctl, &S.win[(it + 1) & 1], &S.ticket[(it + 1) & 1]);
+        const uint32_t ent = (uint32_t)t < nsub ? win.entries[t] : (uint32_t)kIndexNoEntry;
+        if ((uint32_t)t + kUxThreads < nsub_all && win.entries[t + kUxThreads] != kIndexNoEntry) mismatch = 1;   // no starts beyond piece 255
+        S.landed[t] = 0;
+        map4[2 * t] = make_uint4(0, 0, 0, 0);
+        map4[2 * t + 1] = make_uint4(0, 0, 0, 0);
+        hap_mbar_wait(&S.bar, phase);
+        phase ^= 1;
+        __syncthreads();
+        HAP_PHASE_MARK(kPhStage);
+        const uint32_t coff = (uint32_t)((uintptr_t)(src + win.in_off) & 15);
+        const uint8_t *cin = S.cin + coff;
+        const uint32_t wb = win.in_off;
+
+        // ---- walk: every entered piece from its entry to its end (as the execute kernel's walk, for a self-contained fragment)
+        const uint32_t my_lo = (uint32_t)t * sub;
+        const uint32_t my_hi = ((uint32_t)t + 1 == nsub) ? win.in_len : ((uint32_t)t + 1) * sub;
+        const bool entered = (uint32_t)t < nsub && ent != kIndexNoEntry;
+        WalkResult wr;
+        wr.exit = 0; wr.count = 0; wr.out_bytes = 0; wr.invalid = 0; wr.coarse = 0;
+        if (entered) {
+            if (my_lo + ent >= my_hi) {
+                wr.invalid = 1;
+            } else {
+                wr = walk_piece(cin, wb, my_lo + ent, my_hi, in_end);
+                if (!wr.invalid && wr.exit < win.in_len) {
+                    uint32_t b = wr.exit >> win.sub_log2;
+                    b = b < (uint32_t)kUxThreads ? b : (uint32_t)kUxThreads - 1;
+                    S.landed[b] = 1;
+                    if (b * sub + win.entries[b] != wr.exit) mismatch = 1;
+                }
+                if (wr.exit > win.in_len) wr.invalid = 1;
+            }
+        }
+        HAP_PHASE_MARK(kPhWalk);
+        uint32_t total_o;
+        const uint32_t obase = block_excl_sum<kUxThreads>(wr.out_bytes > 0x40000000u ? 0x40000000u : wr.out_bytes, &total_o, S.scratch);
+        // the entries must describe exactly the chain that starts at byte 0 of the fragment (see the execute kernel)
+        const bool should = (uint32_t)t < nsub && (t == 0 || S.landed[t]);
+        int bad = wr.invalid || should != entered || (t == 0 && (!entered || ent != 0)) || total_o != win.out_len;
+        bad = __syncthreads_or(bad || mismatch);
+        const bool coarse = __syncthreads_or(wr.coarse != 0) != 0;
+        HAP_PHASE_MARK(kPhScan);
+        if (bad) {
+            if (t == 0) { job.status = kStatusIndexMismatch; done[w] = 1u; }
+            continue;
+        }
+        if (coarse) {
+            // not 8-byte granular: the execute kernel decodes this window (its tickets reach chunk window k)
+            if (t == 0) {
+                atomicMax(&ctl->max_k_rest, w - job.win_base + 1);
+#ifdef HAPB200_EMU
+                emu_unit_kernel_declined()++;
+#endif
+            }
+            continue;
+        }
+
+        // ---- records: one per element at its first unit (kUnitLit + stream position of a literal, the copy's distance in units)
+        int crossing = 0;
+        if (entered) {
+            uint32_t u = obase >> 3, pos = my_lo + ent;   // (obase is a multiple of 8: every element before this piece is)
+            while (pos < my_hi) {
+                uint32_t len, aux, hdr, kind;
+                read_element_header(cin + pos, wb + pos, in_end, len, aux, hdr, kind);   // (the walk checked every header)
+                if (kind == 0) {
+                    S.map[u] = (uint16_t)(kUnitLit + (aux - wb));
+                    pos += hdr + len;
+                } else {
+                    const uint32_t d = aux >> 3;
+                    if (d > u) { crossing = 1; break; }   // reads before the fragment: the repair pass decodes the chunk
+                    S.map[u] = (uint16_t)d;
+                    pos += hdr;
+                }
+                u += len >> 3;
+            }
+        }
+        if (__syncthreads_or(crossing)) {
+            if (t == 0) { job.status = kStatusIndexMismatch; done[w] = 1u; }
+            continue;
+        }
+        HAP_PHASE_MARK(kPhRecords);
+
+        // ---- map: thread t owns units 16t .. 16t + 15.  The element running into the strip comes from a max-scan over
+        //      (unit + 1) << 16 | record of the strip's last element start; the unit's source then follows by counting.
+        const uint32_t U = win.out_len >> 3, u0 = kUnitStripLen * (uint32_t)t;
+        uint32_t r[kUnitStripLen];
+        {
+            const uint4 a = map4[2 * t], b = map4[2 * t + 1];
+            const uint32_t wd[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+#pragma unroll
+            for (int k = 0; k < kUnitStripLen; k++) r[k] = (wd[k >> 1] >> (16 * (k & 1))) & 0xFFFFu;
+        }
+        uint32_t last = 0;
+#pragma unroll
+        for (int k = 0; k < kUnitStripLen; k++) last = r[k] != 0 ? ((u0 + k + 1) << 16) | r[k] : last;
+        uint32_t unused;
+        const uint32_t carry = block_excl_max<kUxThreads>(last, &unused, S.scratch);   // ends with a barrier: the records are read
+        // v: the source of the current unit; per: the copy's period (distance), 0 for a literal; q: units since the period began
+        uint32_t v = 0, per = 0, q = 0, step = 0;
+        if (carry) {
+            const uint32_t start = (carry >> 16) - 1, rs = carry & 0xFFFFu, d = u0 - start;
+            if (rs >= kUnitLit) { v = rs + 8 * d; step = 8; per = 0; }
+            else { per = rs; q = d % rs; v = start - rs + q; step = 1; }
+        }
+        int pending = 0;
+        uint32_t m[kUnitStripLen];
+#pragma unroll
+        for (int k = 0; k < kUnitStripLen; k++) {
+            const uint32_t u = u0 + k;
+            if (r[k] != 0) {
+                if (r[k] >= kUnitLit) { v = r[k]; step = 8; per = 0; }
+                else { per = r[k]; q = 0; v = u - per; step = 1; }
+            } else if (k > 0) {   // (k == 0: v, q are those of unit u0 already)
+                v += step;
+                if (per != 0 && ++q == per) { q = 0; v -= per; }
+            }
+            m[k] = v;
+            pending |= u < U && v < kUnitLit;
+        }
+#pragma unroll
+        for (int h = 0; h < 2; h++)
+            map4[2 * t + h] = make_uint4((m[8 * h] & 0xFFFFu) | (m[8 * h + 1] << 16), (m[8 * h + 2] & 0xFFFFu) | (m[8 * h + 3] << 16),
+                                         (m[8 * h + 4] & 0xFFFFu) | (m[8 * h + 5] << 16), (m[8 * h + 6] & 0xFFFFu) | (m[8 * h + 7] << 16));
+        pending = __syncthreads_or(pending);
+        HAP_PHASE_MARK(kPhMap);
+
+        // ---- resolve: map[u] = map[map[u]] until every unit names stream bytes (sources are strictly earlier units)
+        for (int round = 0; pending; round++) {
+            pending = 0;
+            for (uint32_t u = t; u < U; u += kUxThreads) {
+                const uint32_t x = S.map[u];
+                if (x < kUnitLit) {
+                    const uint32_t x2 = S.map[x];
+                    S.map[u] = (uint16_t)x2;
+                    pending |= x2 < kUnitLit;
+                }
+            }
+            pending = __syncthreads_or(pending);
+            HAP_PHASE_MARK(kPhRounds);
+            HAP_PHASE_COUNT(kPhRoundCount);
+            if (pending && round == kUnitMaxRounds) { crossing = 1; break; }   // (cannot happen: chains are at most 4096 units deep)
+        }
+        if (crossing) {
+            if (t == 0) { job.status = kStatusIndexMismatch; done[w] = 1u; }
+            continue;
+        }
+
+        // ---- write: thread g assembles destination-aligned 16-byte group g from two or three units of the staged window
+        const uint32_t *c32 = reinterpret_cast<const uint32_t *>(S.cin);
+        const uint32_t mis = (uint32_t)((uintptr_t)out & 15);
+        const uint32_t ngroups = (mis + win.out_len + 15) >> 4;
+        for (uint32_t g = t; g < ngroups; g += kUxThreads) {
+            const int32_t x = 16 * (int32_t)g - (int32_t)mis;
+            const int32_t ua = x >> 3;   // (floor: -2 or -1 for the first group of a misaligned fragment)
+            const uint32_t rr = (uint32_t)x & 7u;
+            uint32_t wv[6];
+#pragma unroll
+            for (int k = 0; k < 3; k++) {
+                const int32_t u = ua + k;
+                wv[2 * k] = 0;
+                wv[2 * k + 1] = 0;
+                if (u >= 0 && (uint32_t)u < U && (k < 2 || rr != 0)) {
+                    const uint32_t b = coff + (uint32_t)S.map[u] - kUnitLit, i = b >> 2, sh = 8 * (b & 3);
+                    const uint32_t s0 = c32[i], s1 = c32[i + 1], s2 = c32[i + 2];
+                    wv[2 * k] = __funnelshift_r(s0, s1, sh);
+                    wv[2 * k + 1] = __funnelshift_r(s1, s2, sh);
+                }
+            }
+            const uint32_t qq = rr >> 2, sh = 8 * (rr & 3);
+            const uint32_t o0 = __funnelshift_r(wv[qq], wv[qq + 1], sh), o1 = __funnelshift_r(wv[qq + 1], wv[qq + 2], sh);
+            const uint32_t o2 = __funnelshift_r(wv[qq + 2], wv[qq + 3], sh), o3 = __funnelshift_r(wv[qq + 3], wv[qq + 4], sh);
+            if (x >= 0 && (uint32_t)x + 16 <= win.out_len) {
+                *reinterpret_cast<uint4 *>(out + x) = make_uint4(o0, o1, o2, o3);   // 16-byte aligned by the choice of mis
+            } else {
+                const uint32_t ow[4] = {o0, o1, o2, o3};
+                for (int i = 0; i < 16; i++)
+                    if (x + i >= 0 && (uint32_t)(x + i) < win.out_len) out[x + i] = (uint8_t)(ow[i >> 2] >> (8 * (i & 3)));
+            }
+        }
+        if (t == 0) {
+            done[w] = 1u;
+#ifdef HAPB200_EMU
+            emu_unit_kernel_windows()++;
+#endif
+        }
+        HAP_PHASE_MARK(kPhWrite);
+        HAP_PHASE_COUNT(kPhUnitWindows);
+    }
+    HAP_PHASE_END();
 }
 
 }  // namespace hapb200

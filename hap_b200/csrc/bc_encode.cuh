@@ -1,4 +1,5 @@
-// hap_b200/csrc/bc_encode.cuh -- K1-K4 kernels: RGBA8 (or NV12 / P010) frames -> DXT1 / DXT5 / scaled-YCoCg-DXT5 / RGTC1 blocks.
+// hap_b200/csrc/bc_encode.cuh -- K1-K4 kernels: RGBA8 (or NV12 / P010, or planar Y'CbCr) frames -> DXT1 / DXT5 /
+// scaled-YCoCg-DXT5 / RGTC1 blocks.
 //
 // One thread per 4x4 block (see bc_block.cuh for why).  Memory shape: thread t of a warp owns block
 // column bx0+t, so for each of the four pixel rows the warp reads 32 x 16 B = 512 contiguous bytes
@@ -73,28 +74,17 @@ __device__ __forceinline__ void load_block_rgba8(const uint8_t *pic, uint32_t ro
 // The frame is blockIdx.y, and gridDim.y is at most 65535: batches of more frames are launched in slices of this many.
 constexpr uint32_t kBcFramesPerLaunch = 65535;
 
-// grid = (bc_ctas, frames).  REFINE: the chroma endpoint refinement of the YCoCg kinds (bc_block.cuh).  kBcBc7 asks for one
-// resident CTA (a cap of 255 registers): its exact-error search holds more state than any register cap would keep.
-// SRC (BcSource): kSrcRgba8 reads `rgba` as RGBA8 rows; kSrcNv12 / kSrcP010 read it as the luma plane and Y.chroma as the
-// chroma plane (yuv_source.cuh), both frame_bytes apart per frame, and convert before the fit.  Y comes last so that the
-// parameters of the RGBA8 instantiations keep their offsets.
-template <int KIND, bool REFINE = false, int SRC = kSrcRgba8>
-__global__ void __launch_bounds__(kBcThreads, (KIND == kBcYCoCg && !REFINE) ? 7 : (KIND == kBcDxt1 || KIND == kBcDxt5) ? 5 : KIND == kBcBc7 ? 1 : HAPB200_BC_MIN_BLOCKS) bc_encode_kernel(const uint8_t *__restrict__ rgba, BcGeom G,
-                                                                uint8_t *__restrict__ out, YuvSrc Y = YuvSrc())
+// Resident CTAs each kind asks for (= its register cap).  kBcBc7 asks for one (a cap of 255 registers): its exact-error
+// search holds more state than any register cap would keep.
+constexpr int bc_encode_min_ctas(int kind, bool refine)
 {
-    const uint32_t nblocks = G.blocks_x * G.blocks_y;
-    const uint32_t bi = blockIdx.x * kBcThreads + threadIdx.x;
-    if (bi >= nblocks) return;
-    uint32_t bx, by;
-    block_xy(bi, G.blocks_x, G.inv_blocks_x, bx, by);
-    uint32_t px[16];
-    if (SRC == kSrcRgba8) {
-        load_block_rgba8(rgba + (uint64_t)blockIdx.y * G.frame_bytes, G.row_bytes, bx, by, px);
-    } else {
-        const uint64_t f = (uint64_t)blockIdx.y * G.frame_bytes;
-        load_block_yuv<SRC>(rgba + f, Y.chroma + f, G.row_bytes, bx, by, G.blocks_x, G.blocks_y, Y, px);
-    }
-    uint8_t *o = out + (uint64_t)blockIdx.y * G.out_stride;
+    return (kind == kBcYCoCg && !refine) ? 7 : (kind == kBcDxt1 || kind == kBcDxt5) ? 5 : kind == kBcBc7 ? 1 : HAPB200_BC_MIN_BLOCKS;
+}
+
+// The fit of block bi from its texels px and its store into this frame's output o (both encode kernels)
+template <int KIND, bool REFINE>
+__device__ __forceinline__ void bc_encode_store(const uint32_t px[16], const BcGeom &G, uint8_t *o, uint32_t bi)
+{
     if (KIND == kBcDxt1) {
         Block8 c = encode_dxt1(px);
         reinterpret_cast<uint2 *>(o)[bi] = make_uint2(c.lo, c.hi);
@@ -118,6 +108,52 @@ __global__ void __launch_bounds__(kBcThreads, (KIND == kBcYCoCg && !REFINE) ? 7 
             reinterpret_cast<uint2 *>(o + G.second_offset)[bi] = make_uint2(al.lo, al.hi);
         }
     }
+}
+
+// grid = (bc_ctas, frames).  REFINE: the chroma endpoint refinement of the YCoCg kinds (bc_block.cuh).
+// SRC (BcSource): kSrcRgba8 reads `rgba` as RGBA8 rows; kSrcNv12 / kSrcP010 read it as the luma plane and Y.chroma as the
+// chroma plane (yuv_source.cuh), both frame_bytes apart per frame, and convert before the fit.  Y comes last so that the
+// parameters of the RGBA8 instantiations keep their offsets.
+template <int KIND, bool REFINE = false, int SRC = kSrcRgba8>
+__global__ void __launch_bounds__(kBcThreads, bc_encode_min_ctas(KIND, REFINE)) bc_encode_kernel(const uint8_t *__restrict__ rgba, BcGeom G,
+                                                                uint8_t *__restrict__ out, YuvSrc Y = YuvSrc())
+{
+    const uint32_t nblocks = G.blocks_x * G.blocks_y;
+    const uint32_t bi = blockIdx.x * kBcThreads + threadIdx.x;
+    if (bi >= nblocks) return;
+    uint32_t bx, by;
+    block_xy(bi, G.blocks_x, G.inv_blocks_x, bx, by);
+    uint32_t px[16];
+    if (SRC == kSrcRgba8) {
+        load_block_rgba8(rgba + (uint64_t)blockIdx.y * G.frame_bytes, G.row_bytes, bx, by, px);
+    } else {
+        const uint64_t f = (uint64_t)blockIdx.y * G.frame_bytes;
+        load_block_yuv<SRC>(rgba + f, Y.chroma + f, G.row_bytes, bx, by, G.blocks_x, G.blocks_y, Y, px);
+    }
+    bc_encode_store<KIND, REFINE>(px, G, out + (uint64_t)blockIdx.y * G.out_stride, bi);
+}
+
+// The same kernel for the planar sources (SRC: kSrcPlanar*, yuv_source.cuh): `luma` is the luma plane, P holds the chroma
+// and alpha planes, all frame_bytes apart per frame.  A kernel of its own, so that the parameters, and so the -Xptxas -v
+// lines, of bc_encode_kernel's instantiations stay as they are.  KIND kBcRgtc1 reads the alpha plane alone.
+template <int KIND, bool REFINE, int SRC>
+__global__ void __launch_bounds__(kBcThreads, bc_encode_min_ctas(KIND, REFINE)) bc_encode_planar_kernel(const uint8_t *__restrict__ luma, BcGeom G,
+                                                                       uint8_t *__restrict__ out, PlanarSrc P)
+{
+    const uint32_t nblocks = G.blocks_x * G.blocks_y;
+    const uint32_t bi = blockIdx.x * kBcThreads + threadIdx.x;
+    if (bi >= nblocks) return;
+    uint32_t bx, by;
+    block_xy(bi, G.blocks_x, G.inv_blocks_x, bx, by);
+    const uint64_t f = (uint64_t)blockIdx.y * G.frame_bytes;
+    PlanarSrc p = P;
+    p.m.chroma += f;
+    p.cr += f;
+    if (p.alpha) p.alpha += f;
+    uint32_t px[16];
+    constexpr bool kAlpha = KIND == kBcDxt5 || KIND == kBcYCoCgPlusAlpha || KIND == kBcRgtc1;
+    load_block_planar<SRC, KIND != kBcRgtc1, kAlpha>(luma + f, G.row_bytes, bx, by, G.blocks_x, G.blocks_y, p, px);
+    bc_encode_store<KIND, REFINE>(px, G, out + (uint64_t)blockIdx.y * G.out_stride, bi);
 }
 
 }  // namespace hapb200

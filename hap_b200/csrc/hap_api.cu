@@ -409,16 +409,57 @@ void launch_bc_encode_slice(const dim3 &grid, cudaStream_t st, const uint8_t *sr
     else HAP_KLAUNCH(kStBcEncode, (bc_encode_kernel<KIND, false, SRC>), grid, dim3(kBcThreads), 0, st, src, g, dst, yuv);
 }
 
-// One launch per kBcFramesPerLaunch frames.  The kinds that encode colour (not RGTC1 alone, not BC7) also read NV12 / P010.
+// the planar sources' kernel (bc_encode_planar_kernel), as launch_bc_encode_slice
+template <int KIND, int SRC>
+void launch_bc_encode_planar_slice(const dim3 &grid, cudaStream_t st, const uint8_t *luma, const BcGeom &g, uint8_t *dst, bool refine,
+                                   const PlanarSrc &p)
+{
+    constexpr bool kRefines = KIND == kBcYCoCg || KIND == kBcYCoCgPlusAlpha;
+    if (kRefines && refine) HAP_KLAUNCH(kStBcEncode, (bc_encode_planar_kernel<KIND, kRefines, SRC>), grid, dim3(kBcThreads), 0, st, luma, g, dst, p);
+    else HAP_KLAUNCH(kStBcEncode, (bc_encode_planar_kernel<KIND, false, SRC>), grid, dim3(kBcThreads), 0, st, luma, g, dst, p);
+}
+
+// RGTC1 (Hap Alpha-Only) reads the alpha plane alone, so only the sample width picks its instantiation
+template <int KIND>
+void launch_bc_encode_planar(const dim3 &grid, cudaStream_t st, const uint8_t *luma, const BcGeom &g, uint8_t *dst, bool refine, int src,
+                             const PlanarSrc &p)
+{
+    if constexpr (KIND == kBcRgtc1) {
+        if (planar_wide(src)) launch_bc_encode_planar_slice<KIND, kSrcPlanar420x16>(grid, st, luma, g, dst, refine, p);
+        else launch_bc_encode_planar_slice<KIND, kSrcPlanar420x8>(grid, st, luma, g, dst, refine, p);
+    } else {
+        switch (src) {
+        case kSrcPlanar420x8: launch_bc_encode_planar_slice<KIND, kSrcPlanar420x8>(grid, st, luma, g, dst, refine, p); break;
+        case kSrcPlanar420x16: launch_bc_encode_planar_slice<KIND, kSrcPlanar420x16>(grid, st, luma, g, dst, refine, p); break;
+        case kSrcPlanar422x8: launch_bc_encode_planar_slice<KIND, kSrcPlanar422x8>(grid, st, luma, g, dst, refine, p); break;
+        case kSrcPlanar422x16: launch_bc_encode_planar_slice<KIND, kSrcPlanar422x16>(grid, st, luma, g, dst, refine, p); break;
+        case kSrcPlanar444x8: launch_bc_encode_planar_slice<KIND, kSrcPlanar444x8>(grid, st, luma, g, dst, refine, p); break;
+        default: launch_bc_encode_planar_slice<KIND, kSrcPlanar444x16>(grid, st, luma, g, dst, refine, p); break;
+        }
+    }
+}
+
+// One launch per kBcFramesPerLaunch frames.  The kinds that encode colour (not RGTC1 alone, not BC7) also read NV12 / P010;
+// the planar sources serve every kind but BC7.
 template <int KIND>
 void launch_bc_encode(uint32_t frames, cudaStream_t st, const uint8_t *rgba, const BcGeom &g, uint8_t *blocks, bool refine, int src,
-                      const YuvSrc &yuv)
+                      const YuvSrc &yuv, const PlanarSrc &planar)
 {
     constexpr bool kTakesYuv = KIND != kBcRgtc1 && KIND != kBcBc7;
     for (uint32_t f0 = 0; f0 < frames; f0 += kBcFramesPerLaunch) {
         const dim3 grid(bc_ctas(g.blocks_x, g.blocks_y), frames - f0 < kBcFramesPerLaunch ? frames - f0 : kBcFramesPerLaunch);
         const uint8_t *s = rgba + f0 * g.frame_bytes;
         uint8_t *dst = blocks + f0 * g.out_stride;
+        if constexpr (KIND != kBcBc7) {
+            if (is_planar_src(src)) {
+                PlanarSrc p = planar;
+                p.m.chroma += f0 * g.frame_bytes;
+                p.cr += f0 * g.frame_bytes;
+                if (p.alpha) p.alpha += f0 * g.frame_bytes;
+                launch_bc_encode_planar<KIND>(grid, st, s, g, dst, refine, src, p);
+                continue;
+            }
+        }
         YuvSrc y = yuv;
         if (y.chroma) y.chroma += f0 * g.frame_bytes;
         if constexpr (kTakesYuv) {
@@ -430,21 +471,24 @@ void launch_bc_encode(uint32_t frames, cudaStream_t st, const uint8_t *rgba, con
 }
 
 // src (BcSource): kSrcRgba8 reads `rgba` as RGBA8 rows row_bytes apart; kSrcNv12 / kSrcP010 read it as the luma plane and
-// yuv.chroma as the chroma plane, both with pitch row_bytes.
+// yuv.chroma as the chroma plane, both with pitch row_bytes; kSrcPlanar* read it as the luma plane (rows row_bytes apart)
+// and `planar` for the others.
 uint32_t launch_block_encode(const uint8_t *rgba, uint32_t frames, uint64_t frame_stride, uint32_t width, uint32_t height,
                              uint64_t row_bytes, const CodecInfo &ci, uint8_t *blocks, uint64_t blocks_stride,
-                             uint64_t second_offset, cudaStream_t st, int src = kSrcRgba8, const YuvSrc &yuv = YuvSrc())
+                             uint64_t second_offset, cudaStream_t st, int src = kSrcRgba8, const YuvSrc &yuv = YuvSrc(),
+                             const PlanarSrc &planar = PlanarSrc())
 {
     const BcGeom g = bc_encode_geom(width, height, (uint32_t)row_bytes, frame_stride, blocks_stride, second_offset);   // (rgba_geometry_ok: row_bytes < 2^32)
     const bool refine = g_chroma_refine.load() != 0;
-    if (src != kSrcRgba8 && (ci.bc_kind == kBcRgtc1 || ci.bc_kind == kBcBc7)) return HapResult_Bad_Arguments;
+    if (src != kSrcRgba8 && ci.bc_kind == kBcBc7) return HapResult_Bad_Arguments;
+    if ((src == kSrcNv12 || src == kSrcP010) && ci.bc_kind == kBcRgtc1) return HapResult_Bad_Arguments;
     switch (ci.bc_kind) {
-    case kBcDxt1: launch_bc_encode<kBcDxt1>(frames, st, rgba, g, blocks, refine, src, yuv); break;
-    case kBcDxt5: launch_bc_encode<kBcDxt5>(frames, st, rgba, g, blocks, refine, src, yuv); break;
-    case kBcYCoCg: launch_bc_encode<kBcYCoCg>(frames, st, rgba, g, blocks, refine, src, yuv); break;
-    case kBcRgtc1: launch_bc_encode<kBcRgtc1>(frames, st, rgba, g, blocks, refine, src, yuv); break;
-    case kBcYCoCgPlusAlpha: launch_bc_encode<kBcYCoCgPlusAlpha>(frames, st, rgba, g, blocks, refine, src, yuv); break;
-    case kBcBc7: launch_bc_encode<kBcBc7>(frames, st, rgba, g, blocks, refine, src, yuv); break;
+    case kBcDxt1: launch_bc_encode<kBcDxt1>(frames, st, rgba, g, blocks, refine, src, yuv, planar); break;
+    case kBcDxt5: launch_bc_encode<kBcDxt5>(frames, st, rgba, g, blocks, refine, src, yuv, planar); break;
+    case kBcYCoCg: launch_bc_encode<kBcYCoCg>(frames, st, rgba, g, blocks, refine, src, yuv, planar); break;
+    case kBcRgtc1: launch_bc_encode<kBcRgtc1>(frames, st, rgba, g, blocks, refine, src, yuv, planar); break;
+    case kBcYCoCgPlusAlpha: launch_bc_encode<kBcYCoCgPlusAlpha>(frames, st, rgba, g, blocks, refine, src, yuv, planar); break;
+    case kBcBc7: launch_bc_encode<kBcBc7>(frames, st, rgba, g, blocks, refine, src, yuv, planar); break;
     default: return HapResult_Bad_Arguments;
     }
     return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
@@ -483,23 +527,40 @@ const uint16_t *pq_table(uint32_t unit_nits, PqDirection dir)
 }
 
 // The picture an encoder reads: an RGBA8 picture (kSrcRgba8), the luma and chroma planes of an NV12 / P010 picture
-// (kSrcNv12 / kSrcP010, yuv_source.cuh), an RGBA16F picture (kSrcRgbaHalf) or an HDR10 P010 picture (kSrcP010Pq).  Rows of
-// both planes are `pitch` bytes apart.
+// (kSrcNv12 / kSrcP010, yuv_source.cuh), an RGBA16F picture (kSrcRgbaHalf), an HDR10 P010 picture (kSrcP010Pq) or a planar
+// picture (kSrcPlanar*).  Rows of the luma (and alpha) plane are `pitch` bytes apart; rows of the NV12 / P010 chroma plane
+// too, rows of the planar chroma planes chroma_pitch bytes apart.
 struct PictureSrc {
     int kind;                 // BcSource
     const void *pixels;       // the RGBA8 / RGBA16F picture, or the luma plane
-    const void *chroma;       // the interleaved CbCr plane
+    const void *chroma;       // the interleaved CbCr plane, or the planar Cb plane
     unsigned color_space;     // HapB200YUVColorSpace
     unsigned unit_nits = 0;   // kSrcP010Pq: the luminance of 1.0
+    // kSrcPlanar*: the Cr and alpha planes (alpha nullptr: A = 255), the chroma planes' pitch and the sample depth.
+    // alpha_only (Hap Alpha-Only): only the alpha plane is read, and pixels, chroma and cr point at it too.
+    const void *cr = nullptr, *alpha = nullptr;
+    uint64_t chroma_pitch = 0;
+    unsigned bit_depth = 0;
+    bool alpha_only = false;
     uint64_t sample_bytes() const   // per pixel of a luma / RGBA row
     {
+        if (is_planar_src(kind)) return planar_wide(kind) ? 2 : 1;
         return kind == kSrcRgba8 ? 4 : kind == kSrcRgbaHalf ? 8 : kind == kSrcNv12 ? 1 : 2;
     }
-    uint32_t planes() const { return kind == kSrcRgba8 || kind == kSrcRgbaHalf ? 1 : 2; }
+    uint32_t planes() const { return kind == kSrcRgba8 || kind == kSrcRgbaHalf ? 1 : is_planar_src(kind) ? 4 : 2; }
     YuvSrc yuv() const
     {
         return kind == kSrcNv12 || kind == kSrcP010 ? yuv_src(kind - kSrcNv12, color_space, (const uint8_t *)chroma) : YuvSrc();
     }
+    PlanarSrc planar() const
+    {
+        return is_planar_src(kind) ? planar_src_args(bit_depth, color_space, (const uint8_t *)chroma, (const uint8_t *)cr,
+                                                     (const uint8_t *)alpha, (uint32_t)chroma_pitch)
+                                   : PlanarSrc();
+    }
+    // the chroma planes' samples per row and rows of a width x height picture
+    uint32_t chroma_width(uint32_t width) const { return planar_subsampling(kind) == HapB200Chroma_444 ? width : width / 2; }
+    uint32_t chroma_height(uint32_t height) const { return planar_subsampling(kind) == HapB200Chroma_420 ? height / 2 : height; }
 };
 PictureSrc rgba_picture(const void *rgba) { return {kSrcRgba8, rgba, nullptr, 0}; }
 PictureSrc rgba_half_picture(const void *rgba) { return {kSrcRgbaHalf, rgba, nullptr, 0}; }
@@ -1363,8 +1424,19 @@ bool yuv_geometry_ok(const void *luma, const void *chroma, unsigned width, unsig
     return chroma && rgba_geometry_ok(luma, width, height, pitch, frameStride, aligned, bpp) && (!aligned || (uintptr_t)chroma % 16 == 0);
 }
 
+// A planar picture's four planes (see PictureSrc): luma (and alpha) as rgba_geometry_ok with `pitch`; Cb and Cr of
+// p.chroma_width(width) samples per row, rows p.chroma_pitch apart.  Alpha-only pictures are checked as their alpha plane.
+bool planar_geometry_ok(const PictureSrc &p, unsigned width, unsigned height, unsigned long pitch, unsigned long frameStride, bool aligned)
+{
+    if (!rgba_geometry_ok(p.pixels, width, height, pitch, frameStride, aligned, p.sample_bytes())) return false;
+    if (p.alpha_only) return true;
+    if (!p.chroma || !p.cr || p.chroma_pitch < p.sample_bytes() * p.chroma_width(width) || p.chroma_pitch > HAPB200_MAX_ROW_BYTES) return false;
+    return !aligned || (((uintptr_t)p.chroma | (uintptr_t)p.cr | (uintptr_t)p.alpha | p.chroma_pitch) % 16 == 0);
+}
+
 bool picture_geometry_ok(const PictureSrc &p, unsigned width, unsigned height, unsigned long pitch, unsigned long frameStride, bool aligned)
 {
+    if (is_planar_src(p.kind)) return planar_geometry_ok(p, width, height, pitch, frameStride, aligned);
     if (p.planes() == 1) return rgba_geometry_ok(p.pixels, width, height, pitch, frameStride, aligned, p.sample_bytes());
     return yuv_geometry_ok(p.pixels, p.chroma, width, height, pitch, frameStride, aligned, p.sample_bytes());
 }
@@ -1380,7 +1452,7 @@ static unsigned block_encode_picture_batch(const CodecInfo &ci, const PictureSrc
     HAP_ENTER(p.pixels, blocks);
     return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
         return launch_block_encode((const uint8_t *)p.pixels, frames, frameStride, width, height, pitch, ci, (uint8_t *)blocks, blocksStride,
-                                   texture_bytes(width, height, ci, 0), st, p.kind, p.yuv());
+                                   texture_bytes(width, height, ci, 0), st, p.kind, p.yuv(), p.planar());
     });
 }
 
@@ -1403,14 +1475,14 @@ static unsigned encode_picture_batch(const CodecInfo &ci, const PictureSrc &p, u
             frames, ci.textures, t, ci.fmt, compressor, chunkCount, (uint8_t *)out, outStride, used, st,
             [&](uint8_t *tex, uint64_t stride) {
                 return launch_block_encode((const uint8_t *)p.pixels, frames, frameStride, width, height, pitch, ci, tex, stride, align16(t[0]),
-                                           st, p.kind, p.yuv());
+                                           st, p.kind, p.yuv(), p.planar());
             },
             fuse ? &fp : nullptr);
     });
 }
 
 // One picture in host or device memory, its arguments checked: its planes are copied into tight device scratch (rows
-// align16(row bytes) apart, chroma after luma) and encoded as a batch of one by
+// align16(row bytes) apart, chroma after luma; planar pictures: Cb, Cr and alpha after luma) and encoded as a batch of one by
 // batch(device picture, its frame stride, its pitch, out, outStride, used, stream).  cap: the frame's size bound.
 extern "C++" {   // (a template, inside the C ABI block)
 template <class Batch>
@@ -1418,22 +1490,44 @@ static unsigned encode_one_picture(const PictureSrc &p, unsigned width, unsigned
                                    void *outputBuffer, unsigned long outputBufferBytes, unsigned long *outputBufferBytesUsed, Batch &&batch)
 {
     HAP_ENTER(p.pixels, outputBuffer);
-    CallStream call(!is_device(p.pixels) && !is_device(p.chroma) && !is_device(outputBuffer));
+    CallStream call(!is_device(p.pixels) && !is_device(p.chroma) && !is_device(p.cr) && !is_device(p.alpha) && !is_device(outputBuffer));
     cudaStream_t st = call.st;
     DevBuf img(st), frame(st), used(st);
     const uint64_t row = p.sample_bytes() * width, tight = align16(row);   // (RGBA8, RGBA16F: tight = row, width is a multiple of 4)
-    const uint64_t luma_bytes = tight * height, plane_bytes = luma_bytes + (p.planes() == 2 ? tight * (height / 2) : 0);
-    if (!img.alloc(plane_bytes) || !frame.alloc(align16(cap)) || !used.alloc(32)) { cudaGetLastError(); return HapResult_Internal_Error; }
+    // the planes to copy: {source, its pitch, row bytes, rows, tight pitch, where the device copy's pointer goes}
+    struct Plane { const void *from; uint64_t pitch, row, rows, tight; const void **to; };
     PictureSrc dev = p;
-    dev.pixels = img.p;
-    if (cudaMemcpy2DAsync(img.p, tight, p.pixels, pitch, row, height, cudaMemcpyDefault, st) != cudaSuccess) { cudaGetLastError(); return HapResult_Internal_Error; }
-    if (p.planes() == 2) {
-        dev.chroma = img.as<uint8_t>() + luma_bytes;
-        if (cudaMemcpy2DAsync(img.as<uint8_t>() + luma_bytes, tight, p.chroma, pitch, row, height / 2, cudaMemcpyDefault, st) != cudaSuccess) {
+    Plane planes[4];
+    int n = 0;
+    if (is_planar_src(p.kind)) {
+        const uint64_t crow = p.sample_bytes() * (p.alpha_only ? 0 : p.chroma_width(width)), ctight = align16(crow);
+        dev.chroma_pitch = ctight;
+        if (p.alpha_only) {
+            planes[n++] = {p.alpha, pitch, row, height, tight, &dev.alpha};
+        } else {
+            planes[n++] = {p.pixels, pitch, row, height, tight, &dev.pixels};
+            planes[n++] = {p.chroma, p.chroma_pitch, crow, p.chroma_height(height), ctight, &dev.chroma};
+            planes[n++] = {p.cr, p.chroma_pitch, crow, p.chroma_height(height), ctight, &dev.cr};
+            if (p.alpha) planes[n++] = {p.alpha, pitch, row, height, tight, &dev.alpha};
+        }
+    } else {
+        planes[n++] = {p.pixels, pitch, row, height, tight, &dev.pixels};
+        if (p.planes() == 2) planes[n++] = {p.chroma, pitch, row, height / 2, tight, &dev.chroma};
+    }
+    uint64_t plane_bytes = 0;
+    for (int i = 0; i < n; i++) plane_bytes += planes[i].tight * planes[i].rows;
+    if (!img.alloc(plane_bytes) || !frame.alloc(align16(cap)) || !used.alloc(32)) { cudaGetLastError(); return HapResult_Internal_Error; }
+    uint64_t at = 0;
+    for (int i = 0; i < n; i++) {
+        const Plane &q = planes[i];
+        *q.to = img.as<uint8_t>() + at;
+        if (cudaMemcpy2DAsync(img.as<uint8_t>() + at, q.tight, q.from, q.pitch, q.row, q.rows, cudaMemcpyDefault, st) != cudaSuccess) {
             cudaGetLastError();
             return HapResult_Internal_Error;
         }
+        at += q.tight * q.rows;
     }
+    if (dev.alpha_only) dev.pixels = dev.chroma = dev.cr = dev.alpha;
     uint32_t r = batch(dev, align16(plane_bytes), tight, frame.p, align16(cap), used.as<unsigned long long>(), st);
     if (r != HapResult_No_Error) return r;
     unsigned long long total = 0;
@@ -1605,6 +1699,67 @@ unsigned int HapB200BlockEncodeYUVBatch(const void *luma, const void *chroma, un
     if (!yuv_args_ok(layout, colorSpace, codec, ci)) return HapResult_Bad_Arguments;
     return block_encode_picture_batch(ci, yuv_picture(luma, chroma, layout, colorSpace), frames, frameStride, width, height, pitch, blocks,
                                       blocksStride, stream);
+}
+
+// ---- planar Y'CbCr 4:2:0 / 4:2:2 / 4:4:4 (+ alpha) -> Hap, Hap Alpha, Hap Q, Hap Q Alpha, Hap Alpha-Only: the picture
+// encoders with a planar source (yuv_source.cuh) ----------------------------------------------------------------------------
+
+// the codecs (every one with a block compressor; HapA only with an alpha plane), subsamplings, depths and colour spaces the
+// planar encoders take
+static bool planar_args_ok(const void *alpha, unsigned subsampling, unsigned bitDepth, unsigned colorSpace, unsigned codec, CodecInfo &ci)
+{
+    return subsampling <= HapB200Chroma_444 && (bitDepth == 8 || bitDepth == 10 || bitDepth == 12) && colorSpace <= HapB200YUV_BT709_Full &&
+           codec_info(codec, ci) && codec_encodes(ci) && (ci.bc_kind != kBcRgtc1 || alpha);
+}
+
+// Hap1 and HapY do not read alpha; HapA reads alpha alone (the picture's other planes are the alpha plane, never read)
+static PictureSrc planar_picture(const CodecInfo &ci, const void *luma, const void *cb, const void *cr, const void *alpha,
+                                 unsigned long chromaPitch, unsigned subsampling, unsigned bitDepth, unsigned colorSpace)
+{
+    PictureSrc p{planar_src(subsampling, bitDepth > 8), luma, cb, colorSpace};
+    p.cr = cr;
+    p.alpha = ci.bc_kind == kBcDxt1 || ci.bc_kind == kBcYCoCg ? nullptr : alpha;
+    p.chroma_pitch = chromaPitch;
+    p.bit_depth = bitDepth;
+    if (ci.bc_kind == kBcRgtc1) {
+        p.alpha_only = true;
+        p.pixels = p.chroma = p.cr = alpha;
+    }
+    return p;
+}
+
+unsigned int HapB200EncodePlanar(const void *luma, const void *cb, const void *cr, const void *alpha, unsigned int width, unsigned int height,
+                                 unsigned long lumaPitch, unsigned long chromaPitch, unsigned int subsampling, unsigned int bitDepth,
+                                 unsigned int colorSpace, unsigned int codec, unsigned int compressor, unsigned int chunkCount,
+                                 void *outputBuffer, unsigned long outputBufferBytes, unsigned long *outputBufferBytesUsed)
+{
+    CodecInfo ci;
+    if (!planar_args_ok(alpha, subsampling, bitDepth, colorSpace, codec, ci)) return HapResult_Bad_Arguments;
+    return encode_picture(ci, planar_picture(ci, luma, cb, cr, alpha, chromaPitch, subsampling, bitDepth, colorSpace), width, height, lumaPitch,
+                          compressor, chunkCount, outputBuffer, outputBufferBytes, outputBufferBytesUsed);
+}
+
+unsigned int HapB200EncodePlanarBatch(const void *luma, const void *cb, const void *cr, const void *alpha, unsigned int frames,
+                                      unsigned long frameStride, unsigned int width, unsigned int height, unsigned long lumaPitch,
+                                      unsigned long chromaPitch, unsigned int subsampling, unsigned int bitDepth, unsigned int colorSpace,
+                                      unsigned int codec, unsigned int compressor, unsigned int chunkCount, void *out, unsigned long outStride,
+                                      unsigned long long *used, void *stream)
+{
+    CodecInfo ci;
+    if (!planar_args_ok(alpha, subsampling, bitDepth, colorSpace, codec, ci)) return HapResult_Bad_Arguments;
+    return encode_picture_batch(ci, planar_picture(ci, luma, cb, cr, alpha, chromaPitch, subsampling, bitDepth, colorSpace), frames, frameStride,
+                                width, height, lumaPitch, compressor, chunkCount, out, outStride, used, stream);
+}
+
+unsigned int HapB200BlockEncodePlanarBatch(const void *luma, const void *cb, const void *cr, const void *alpha, unsigned int frames,
+                                           unsigned long frameStride, unsigned int width, unsigned int height, unsigned long lumaPitch,
+                                           unsigned long chromaPitch, unsigned int subsampling, unsigned int bitDepth, unsigned int colorSpace,
+                                           unsigned int codec, void *blocks, unsigned long blocksStride, void *stream)
+{
+    CodecInfo ci;
+    if (!planar_args_ok(alpha, subsampling, bitDepth, colorSpace, codec, ci)) return HapResult_Bad_Arguments;
+    return block_encode_picture_batch(ci, planar_picture(ci, luma, cb, cr, alpha, chromaPitch, subsampling, bitDepth, colorSpace), frames,
+                                      frameStride, width, height, lumaPitch, blocks, blocksStride, stream);
 }
 
 unsigned int HapB200DecodeBatch(const void *in, unsigned int frames, unsigned long inStride, const unsigned long long *inBytes,

@@ -17,6 +17,7 @@ HapB200YUV_BT601_Limited, HapB200YUV_BT601_Full, HapB200YUV_BT709_Limited, HapB2
 # BT.2020: taken only by the HDR10 encoders (encode_yuv_pq, encode_yuv_pq_batch, block_encode_yuv_pq_batch) and decoders
 # (decode_yuv_pq, decode_yuv_pq_batch, block_decode_yuv_pq_batch)
 HapB200YUV_BT2020_Limited, HapB200YUV_BT2020_Full = 4, 5
+HapB200Chroma_420, HapB200Chroma_422, HapB200Chroma_444 = range(3)
 
 
 def library_path() -> str:
@@ -87,6 +88,12 @@ class HapB200(HapABI):
         L.HapB200EncodeYUVBatch.argtypes = [vp, vp, u, ul, u, u, ul, u, u, u, u, u, vp, ul, vp, vp]
         L.HapB200BlockEncodeYUVBatch.restype = u
         L.HapB200BlockEncodeYUVBatch.argtypes = [vp, vp, u, ul, u, u, ul, u, u, u, vp, ul, vp]
+        L.HapB200EncodePlanar.restype = u
+        L.HapB200EncodePlanar.argtypes = [vp, vp, vp, vp, u, u, ul, ul, u, u, u, u, u, u, vp, ul, C.POINTER(ul)]
+        L.HapB200EncodePlanarBatch.restype = u
+        L.HapB200EncodePlanarBatch.argtypes = [vp, vp, vp, vp, u, ul, u, u, ul, ul, u, u, u, u, u, u, vp, ul, vp, vp]
+        L.HapB200BlockEncodePlanarBatch.restype = u
+        L.HapB200BlockEncodePlanarBatch.argtypes = [vp, vp, vp, vp, u, ul, u, u, ul, ul, u, u, u, u, vp, ul, vp]
         L.HapB200DecodeYUV.restype = u
         L.HapB200DecodeYUV.argtypes = [vp, ul, u, u, vp, vp, ul, u, u]
         L.HapB200DecodeYUVBatch.restype = u
@@ -328,6 +335,46 @@ class HapB200(HapABI):
                                blocks_stride, stream=None):
         return int(self.lib.HapB200BlockEncodeYUVBatch(luma, chroma, frames, frame_stride, w, h, pitch, layout, color_space, codec,
                                                        blocks, blocks_stride, stream))
+
+    # -- planar Y'CbCr (+ alpha) -> Hap, Hap Alpha, Hap Q, Hap Q Alpha, Hap Alpha-Only: subsampling HapB200Chroma_*, bit_depth
+    #    8 / 10 / 12 (10 and 12: little-endian 16-bit words, sample in the low bits), color_space BT.601 / BT.709; luma and alpha
+    #    rows luma_pitch apart (default: width samples), Cb and Cr rows chroma_pitch apart (default: their width in samples);
+    #    alpha None: A = 255; HapA reads alpha alone (luma, cb, cr may be None).  Frames need max_encoded_length_rgba(w, h, codec,
+    #    chunks)
+    @staticmethod
+    def _planar_pitches(w, subsampling, bit_depth, luma_pitch, chroma_pitch):
+        sb = 1 if bit_depth == 8 else 2
+        cw = w if subsampling == HapB200Chroma_444 else w // 2
+        return luma_pitch or sb * w, chroma_pitch or sb * cw
+
+    def encode_planar(self, luma, cb, cr, alpha, w, h, subsampling, bit_depth, color_space, codec, compressor=1, chunks=1,
+                      luma_pitch=None, chroma_pitch=None, out=None, out_capacity=None):
+        """luma, cb, cr, alpha: buffer objects, (addr, nbytes) or None.  Returns (result, frame bytes | used)."""
+        from .abi import _as_ptr
+        addrs = [0 if b is None else _as_ptr(b)[0] for b in (luma, cb, cr, alpha)]
+        lp, cp = self._planar_pitches(w, subsampling, bit_depth, luma_pitch, chroma_pitch)
+        cap = self.max_encoded_length_rgba(w, h, codec, chunks) if out_capacity is None else out_capacity
+        own = out is None
+        if own:
+            out = bytearray(max(cap, 1))
+        oaddr, _ = _as_ptr(out)
+        used = C.c_ulong(0)
+        r = self.lib.HapB200EncodePlanar(*addrs, w, h, lp, cp, subsampling, bit_depth, color_space, codec, compressor, chunks, oaddr,
+                                         cap, C.byref(used))
+        if r != 0:
+            return int(r), None
+        return 0, (bytes(memoryview(out)[: used.value]) if own else used.value)
+
+    def encode_planar_batch(self, luma, cb, cr, alpha, frames, frame_stride, w, h, luma_pitch, chroma_pitch, subsampling, bit_depth,
+                            color_space, codec, compressor, chunks, out, out_stride, used, stream=None):
+        return int(self.lib.HapB200EncodePlanarBatch(luma, cb, cr, alpha, frames, frame_stride, w, h, luma_pitch, chroma_pitch,
+                                                     subsampling, bit_depth, color_space, codec, compressor, chunks, out, out_stride,
+                                                     used, stream))
+
+    def block_encode_planar_batch(self, luma, cb, cr, alpha, frames, frame_stride, w, h, luma_pitch, chroma_pitch, subsampling,
+                                  bit_depth, color_space, codec, blocks, blocks_stride, stream=None):
+        return int(self.lib.HapB200BlockEncodePlanarBatch(luma, cb, cr, alpha, frames, frame_stride, w, h, luma_pitch, chroma_pitch,
+                                                          subsampling, bit_depth, color_space, codec, blocks, blocks_stride, stream))
 
     # -- Hap (every codec but Hap HDR) -> NV12 / P010: layout HapB200YUV_*, color_space BT.601 / BT.709 (no BT.2020); both
     #    planes have the row pitch `pitch` (default: width bytes per sample)

@@ -325,7 +325,74 @@ unsigned int HapB200BlockEncodeYUVBatch(const void *luma, const void *chroma, un
                                         unsigned int colorSpace, unsigned int codec, void *blocks, unsigned long blocksStride,
                                         void *stream);
 
-/* ---- Hap, Hap Alpha, Hap Q, Hap Q Alpha, Hap Alpha-Only, Hap R -> NV12 / P010 ------------------------------------------------
+/* ---- Hap, Hap Alpha, Hap Q, Hap Q Alpha, Hap Alpha-Only <- planar Y'CbCr 4:2:0 / 4:2:2 / 4:4:4 (+ alpha) ---------------------
+ * The encoders take the planar pictures software decoders and mastering formats give (FFmpeg's yuv420p, yuv422p10le,
+ * yuva444p12le and their kin) and convert them to RGBA8 inside the block encoder, so no RGBA picture is ever written.
+ * The arguments follow FFmpeg's AVFrame: luma, cb, cr and alpha are data[0], data[1], data[2] and data[3]; lumaPitch is
+ * linesize[0] and chromaPitch is linesize[1] (= linesize[2]; alpha's rows are lumaPitch apart, as linesize[3] is).
+ * Encoding a planar picture gives exactly the bytes HapB200EncodeRGBA* / HapB200BlockEncodeBatch give for the RGBA8 picture
+ * the conversion below makes of it.
+ * Planes:
+ *   Luma and alpha: width x height samples, rows lumaPitch bytes apart.
+ *   Cb and Cr: cw x ch samples, rows chromaPitch bytes apart; cw = width/2 for 4:2:0 and 4:2:2, width for 4:4:4; ch =
+ *   height/2 for 4:2:0, height otherwise.
+ *   In a batch, each of the four planes of frame f starts at its pointer + f*frameStride.
+ * Samples: bitDepth 8: bytes.  bitDepth 10 or 12: little-endian 16-bit words with the sample in the low bits, as in FFmpeg's
+ *   *p10le / *p12le; the sample is word & (2^n - 1), so higher bits are ignored.  Any other depth is refused.
+ * Geometry: width and height multiples of 4, width*bytes <= lumaPitch <= HAPB200_MAX_ROW_BYTES, cw*bytes <= chromaPitch <=
+ *   HAPB200_MAX_ROW_BYTES (bytes: 1 per sample at 8 bits, else 2), at most HAPB200_MAX_BLOCKS blocks.  The batch entry points
+ *   take device pointers; the planes, both pitches, frameStride, out, outStride, blocks and blocksStride are 16-byte aligned.
+ *   The single-frame call takes host or device memory at any alignment and pitch.
+ * Codecs: HapB200Codec_Hap1 and _HapY do not read alpha.  _Hap5 and _HapM use alpha; a NULL alpha means A = 255.  _HapA
+ *   requires alpha and reads only that plane: luma, cb and cr are neither read nor checked, and may be NULL.  _Hap7 (as for
+ *   every codec-taking encoder) and unknown codecs are refused with HapResult_Bad_Arguments.
+ * Colour spaces: BT.601 and BT.709, limited and full range; BT.2020 is refused, as for HapB200EncodeYUV*.
+ * Every argument is checked before anything touches the GPU.  Sizes (HapB200MaxEncodedLengthRGBA), HapResult_Buffer_Too_Small,
+ * compressor, chunkCount and the index, offset-table and chroma-refine options behave exactly as for HapB200EncodeRGBA*.
+ * The conversion, exactly (n = bitDepth), extending that of HapB200EncodeYUV; chroma keeps its default siting (co-sited
+ * with even luma columns; in 4:2:0 midway between luma rows):
+ *   1. Chroma to eighths, C8 for luma (x, y), row and column indices clamped to the chroma plane:
+ *      4:2:0: exactly HapB200EncodeYUV's upsampler (vertical weights 3 and 1, horizontal weights 2, or 1 and 1).
+ *      4:2:2: vertical weight 4 on row y; for even x weight 2 on column i = x/2, for odd x weight 1 on columns i and i+1.
+ *      4:4:4: C8 = 8*C.
+ *   2. Matrix: n = 8: the NV12 rows of HAPB200_YUV_COEFFICIENTS with shift 16; n = 10: the P010 rows with shift 16 (a 10-bit
+ *      sample has the value P010's word >> 6 has, so both are unchanged).  n = 12: the rows of HAPB200_YUV_12BIT_COEFFICIENTS
+ *      below, each coefficient round(2^18 * 255 * matrix entry / scale), the chroma ones divided by 8 more (limited range:
+ *      luma offset 256, luma scale 3504, chroma scale 3584; full range: offset 0, both scales 4095; chroma offset 2048), with
+ *      R = (cy*Yd + crR*Cr8d + 2^17) >> 18, G and B likewise, each clamped to 0..255.  Every intermediate stays below 2^31.
+ *      The limited rows equal the P010 rows, so 12-bit samples that are 4 times 10-bit ones convert identically.
+ *   3. Alpha: A = (510*a + 2^n - 1) / (2*(2^n - 1)), integer division: 255*a / (2^n - 1) rounded half up (A = a at n = 8).
+ *      Alpha is taken as given: no premultiplication is added or removed. */
+enum HapB200ChromaSubsampling { HapB200Chroma_420 = 0, HapB200Chroma_422 = 1, HapB200Chroma_444 = 2 };
+/* row colorSpace: {cy, crR, cbG, crG, cbB, yOff, cOff}, shift 18 */
+#define HAPB200_YUV_12BIT_COEFFICIENTS                                                                                     \
+    {                                                                                                                      \
+        {19077, 3269, -802, -1665, 4131, 256, 2048},  /* BT.601 limited */                                                 \
+        {16324, 2861, -702, -1457, 3616, 0, 2048},    /* BT.601 full    */                                                 \
+        {19077, 3672, -437, -1091, 4326, 256, 2048},  /* BT.709 limited */                                                 \
+        {16324, 3213, -382, -955, 3786, 0, 2048}      /* BT.709 full    */                                                 \
+    }
+
+/* one picture (host or device pointers, any alignment, any pitches) -> one Hap frame */
+unsigned int HapB200EncodePlanar(const void *luma, const void *cb, const void *cr, const void *alpha,
+                                 unsigned int width, unsigned int height, unsigned long lumaPitch, unsigned long chromaPitch,
+                                 unsigned int subsampling, unsigned int bitDepth, unsigned int colorSpace, unsigned int codec,
+                                 unsigned int compressor, unsigned int chunkCount,
+                                 void *outputBuffer, unsigned long outputBufferBytes, unsigned long *outputBufferBytesUsed);
+/* frames x picture (device) -> frames x Hap frame at out + f*outStride, encoded length in used[f] (device) */
+unsigned int HapB200EncodePlanarBatch(const void *luma, const void *cb, const void *cr, const void *alpha, unsigned int frames,
+                                      unsigned long frameStride, unsigned int width, unsigned int height, unsigned long lumaPitch,
+                                      unsigned long chromaPitch, unsigned int subsampling, unsigned int bitDepth,
+                                      unsigned int colorSpace, unsigned int codec, unsigned int compressor, unsigned int chunkCount,
+                                      void *out, unsigned long outStride, unsigned long long *used, void *stream);
+/* frames x picture (device) -> bare textures, as HapB200BlockEncodeBatch (HapM: RGTC1 plane at blocks + HapB200TextureBytes(.., 0)) */
+unsigned int HapB200BlockEncodePlanarBatch(const void *luma, const void *cb, const void *cr, const void *alpha, unsigned int frames,
+                                           unsigned long frameStride, unsigned int width, unsigned int height,
+                                           unsigned long lumaPitch, unsigned long chromaPitch, unsigned int subsampling,
+                                           unsigned int bitDepth, unsigned int colorSpace, unsigned int codec,
+                                           void *blocks, unsigned long blocksStride, void *stream);
+
+/* ---- Hap, Hap Alpha, Hap Q, Hap Q Alpha, Hap Alpha-Only, Hap R -> NV12 / P010------------------------------------------------
  * The decoders write the 4:2:0 pictures a video encoder takes (NVENC surfaces).  The conversion is fused into the block
  * decoder, so no RGBA picture is ever written.  The planes are exactly the conversion below applied to the RGBA8 picture that
  * HapB200DecodeRGBA / HapB200DecodeRGBABatch / HapB200BlockDecodeBatch give for the same input; alpha is ignored.

@@ -302,6 +302,30 @@ bool codec_info(unsigned codec, CodecInfo &c)
 // the codecs the RGBA encode entry points take: every one with a block compressor (BC7 has none)
 bool codec_encodes(const CodecInfo &c) { return c.bc_kind != kBcBc7; }
 
+// Hap HDR: one BC6H texture, UF16 or SF16 as textureFormat.  No codec value names it (codec_info refuses it): the Hap HDR entry
+// points take the texture format instead.
+constexpr int kBcBc6h = kBcBc7 + 1;
+bool bc6h_codec(unsigned textureFormat, CodecInfo &c)
+{
+    if (textureFormat != HapFmt_RGB_BPTC_UFLOAT && textureFormat != HapFmt_RGB_BPTC_SFLOAT) return false;
+    c = {1, {textureFormat, 0}, {16, 0}, kBcBc6h};
+    return true;
+}
+
+unsigned long texture_bytes(unsigned width, unsigned height, const CodecInfo &ci, unsigned index)
+{
+    if (index >= ci.textures || width % 4 || height % 4) return 0;
+    return (unsigned long)(width / 4) * (height / 4) * ci.block_bytes[index];
+}
+
+unsigned long max_encoded_length_rgba(unsigned width, unsigned height, const CodecInfo &ci, unsigned chunkCount)
+{
+    unsigned long lens[2] = {texture_bytes(width, height, ci, 0), texture_bytes(width, height, ci, 1)};
+    unsigned fmts[2] = {ci.fmt[0], ci.fmt[1]}, chunks[2] = {chunkCount, chunkCount};
+    if (lens[0] == 0) return 0;
+    return HapMaxEncodedLength(ci.textures, lens, fmts, chunks);
+}
+
 // hap.c:551-559 (SURVEY.md Q5): of two textures, one must be scaled YCoCg DXT5 or alpha RGTC1
 bool texture_formats_ok(unsigned count, const unsigned *f)
 {
@@ -470,30 +494,6 @@ void launch_bc_encode(uint32_t frames, cudaStream_t st, const uint8_t *rgba, con
     }
 }
 
-// src (BcSource): kSrcRgba8 reads `rgba` as RGBA8 rows row_bytes apart; kSrcNv12 / kSrcP010 read it as the luma plane and
-// yuv.chroma as the chroma plane, both with pitch row_bytes; kSrcPlanar* read it as the luma plane (rows row_bytes apart)
-// and `planar` for the others.
-uint32_t launch_block_encode(const uint8_t *rgba, uint32_t frames, uint64_t frame_stride, uint32_t width, uint32_t height,
-                             uint64_t row_bytes, const CodecInfo &ci, uint8_t *blocks, uint64_t blocks_stride,
-                             uint64_t second_offset, cudaStream_t st, int src = kSrcRgba8, const YuvSrc &yuv = YuvSrc(),
-                             const PlanarSrc &planar = PlanarSrc())
-{
-    const BcGeom g = bc_encode_geom(width, height, (uint32_t)row_bytes, frame_stride, blocks_stride, second_offset);   // (rgba_geometry_ok: row_bytes < 2^32)
-    const bool refine = g_chroma_refine.load() != 0;
-    if (src != kSrcRgba8 && ci.bc_kind == kBcBc7) return HapResult_Bad_Arguments;
-    if ((src == kSrcNv12 || src == kSrcP010) && ci.bc_kind == kBcRgtc1) return HapResult_Bad_Arguments;
-    switch (ci.bc_kind) {
-    case kBcDxt1: launch_bc_encode<kBcDxt1>(frames, st, rgba, g, blocks, refine, src, yuv, planar); break;
-    case kBcDxt5: launch_bc_encode<kBcDxt5>(frames, st, rgba, g, blocks, refine, src, yuv, planar); break;
-    case kBcYCoCg: launch_bc_encode<kBcYCoCg>(frames, st, rgba, g, blocks, refine, src, yuv, planar); break;
-    case kBcRgtc1: launch_bc_encode<kBcRgtc1>(frames, st, rgba, g, blocks, refine, src, yuv, planar); break;
-    case kBcYCoCgPlusAlpha: launch_bc_encode<kBcYCoCgPlusAlpha>(frames, st, rgba, g, blocks, refine, src, yuv, planar); break;
-    case kBcBc7: launch_bc_encode<kBcBc7>(frames, st, rgba, g, blocks, refine, src, yuv, planar); break;
-    default: return HapResult_Bad_Arguments;
-    }
-    return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
-}
-
 // The PQ tables of the HDR10 converters per (device, direction, unitNits): T of the encoders (kPqIn: yuv_pq_table, 4096
 // halves, 8 KiB) and P of the decoders (kPqOut: yuv_pq_out_table, kPqOutEntries codes, 62 KiB), both of include/hap_b200.h.
 // Built on the host and uploaded by the first call that needs one, which waits for the copy; kept for the life of the
@@ -565,30 +565,57 @@ struct PictureSrc {
 PictureSrc rgba_picture(const void *rgba) { return {kSrcRgba8, rgba, nullptr, 0}; }
 PictureSrc rgba_half_picture(const void *rgba) { return {kSrcRgbaHalf, rgba, nullptr, 0}; }
 
-// RGBA16F / HDR10 P010 pictures (p: kSrcRgbaHalf / kSrcP010Pq, its planes frame_stride apart) -> BC6H blocks (Hap HDR), SF16
-// when is_signed, else UF16.  One launch per kBcFramesPerLaunch frames.
-uint32_t launch_bc6h_encode(const PictureSrc &p, uint32_t frames, uint64_t frame_stride, uint32_t width, uint32_t height, uint64_t row_bytes,
-                            uint8_t *blocks, uint64_t blocks_stride, bool is_signed, cudaStream_t st)
+// The BC6H kind (Hap HDR) of launch_block_encode: RGBA16F pictures (kSrcRgbaHalf) or HDR10 P010 ones (kSrcP010Pq, converted
+// through pq) -> blocks, SF16 when is_signed, else UF16.  One launch per kBcFramesPerLaunch frames.
+void launch_bc6h_slices(uint32_t frames, cudaStream_t st, const uint8_t *rgba, const BcGeom &g, uint8_t *blocks, uint32_t is_signed, int src,
+                        const YuvPqSrc &pq)
 {
-    const BcGeom g = bc_encode_geom(width, height, (uint32_t)row_bytes, frame_stride, blocks_stride, 0);   // (rgba_geometry_ok: row_bytes < 2^32)
-    YuvPqSrc pq = YuvPqSrc();
-    if (p.kind == kSrcP010Pq) {
-        const uint16_t *table = pq_table(p.unit_nits, kPqIn);
-        if (!table) return HapResult_Internal_Error;
-        pq = yuv_pq_src(p.color_space, (const uint8_t *)p.chroma, table);
-    }
-    const uint8_t *src = (const uint8_t *)p.pixels;
     for (uint32_t f0 = 0; f0 < frames; f0 += kBcFramesPerLaunch) {
         const dim3 grid(bc_ctas(g.blocks_x, g.blocks_y), frames - f0 < kBcFramesPerLaunch ? frames - f0 : kBcFramesPerLaunch);
-        if (p.kind == kSrcP010Pq) {
+        if (src == kSrcP010Pq) {
             YuvPqSrc y = pq;
             y.m.chroma += f0 * g.frame_bytes;
-            HAP_KLAUNCH(kStBcEncode, bc6h_encode_kernel<kSrcP010Pq>, grid, dim3(kBcThreads), 0, st, src + f0 * g.frame_bytes, g,
-                        blocks + f0 * g.out_stride, is_signed ? 1u : 0u, y);
+            HAP_KLAUNCH(kStBcEncode, bc6h_encode_kernel<kSrcP010Pq>, grid, dim3(kBcThreads), 0, st, rgba + f0 * g.frame_bytes, g,
+                        blocks + f0 * g.out_stride, is_signed, y);
         } else {
-            HAP_KLAUNCH(kStBcEncode, bc6h_encode_kernel<>, grid, dim3(kBcThreads), 0, st, src + f0 * g.frame_bytes, g, blocks + f0 * g.out_stride,
-                        is_signed ? 1u : 0u, pq);
+            HAP_KLAUNCH(kStBcEncode, bc6h_encode_kernel<>, grid, dim3(kBcThreads), 0, st, rgba + f0 * g.frame_bytes, g, blocks + f0 * g.out_stride,
+                        is_signed, pq);
         }
+    }
+}
+
+// The pictures p (frame f's planes frame_stride apart, luma / RGBA rows row_bytes apart) -> blocks of ci, frame f's at
+// blocks + f*blocks_stride, its second texture (Hap Q Alpha) second_offset behind them.  BC6H signedness: ci.fmt[0].
+uint32_t launch_block_encode(const CodecInfo &ci, const PictureSrc &p, uint32_t frames, uint64_t frame_stride, uint32_t width,
+                             uint32_t height, uint64_t row_bytes, uint8_t *blocks, uint64_t blocks_stride, uint64_t second_offset,
+                             cudaStream_t st)
+{
+    const BcGeom g = bc_encode_geom(width, height, (uint32_t)row_bytes, frame_stride, blocks_stride, second_offset);   // (rgba_geometry_ok: row_bytes < 2^32)
+    const uint8_t *rgba = (const uint8_t *)p.pixels;
+    const int src = p.kind;
+    const YuvSrc yuv = p.yuv();
+    const PlanarSrc planar = p.planar();
+    const bool refine = g_chroma_refine.load() != 0;
+    if (src != kSrcRgba8 && ci.bc_kind == kBcBc7) return HapResult_Bad_Arguments;
+    if ((src == kSrcNv12 || src == kSrcP010) && ci.bc_kind == kBcRgtc1) return HapResult_Bad_Arguments;
+    switch (ci.bc_kind) {
+    case kBcDxt1: launch_bc_encode<kBcDxt1>(frames, st, rgba, g, blocks, refine, src, yuv, planar); break;
+    case kBcDxt5: launch_bc_encode<kBcDxt5>(frames, st, rgba, g, blocks, refine, src, yuv, planar); break;
+    case kBcYCoCg: launch_bc_encode<kBcYCoCg>(frames, st, rgba, g, blocks, refine, src, yuv, planar); break;
+    case kBcRgtc1: launch_bc_encode<kBcRgtc1>(frames, st, rgba, g, blocks, refine, src, yuv, planar); break;
+    case kBcYCoCgPlusAlpha: launch_bc_encode<kBcYCoCgPlusAlpha>(frames, st, rgba, g, blocks, refine, src, yuv, planar); break;
+    case kBcBc7: launch_bc_encode<kBcBc7>(frames, st, rgba, g, blocks, refine, src, yuv, planar); break;
+    case kBcBc6h: {
+        YuvPqSrc pq = YuvPqSrc();
+        if (src == kSrcP010Pq) {
+            const uint16_t *table = pq_table(p.unit_nits, kPqIn);
+            if (!table) return HapResult_Internal_Error;
+            pq = yuv_pq_src(p.color_space, (const uint8_t *)p.chroma, table);
+        }
+        launch_bc6h_slices(frames, st, rgba, g, blocks, ci.fmt[0] == HapFmt_RGB_BPTC_SFLOAT ? 1u : 0u, src, pq);
+        break;
+    }
+    default: return HapResult_Bad_Arguments;
     }
     return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
 }
@@ -621,102 +648,77 @@ uint32_t encode_frames_from_blocks(uint32_t frames, uint32_t count, const uint64
     return launch_encode(tex.as<uint8_t>(), G, frames, out, out_stride, used, st, fused);
 }
 
+// The picture a decoder writes: an RGBA8 picture (kDstRgba8), an RGBA16F picture (kDstRgbaHalf), the luma and chroma planes of
+// an NV12 / P010 picture (kDstNv12 / kDstP010, yuv_sink.cuh) or of an HDR10 P010 picture (kDstP010Pq, BT.2020 PQ).  The
+// chroma plane's rows are as many bytes apart as luma's.
+enum DstKind { kDstRgba8, kDstRgbaHalf, kDstNv12, kDstP010, kDstP010Pq };
+struct PictureDst {
+    int kind;                 // DstKind
+    void *pixels;             // the RGBA8 / RGBA16F picture, or the luma plane
+    void *chroma;             // the interleaved CbCr plane
+    unsigned color_space;     // HapB200YUVColorSpace
+    unsigned unit_nits = 0;   // kDstP010Pq: the luminance of 1.0
+    uint64_t sample_bytes() const   // per pixel of a luma / RGBA row
+    {
+        return kind == kDstRgba8 ? 4 : kind == kDstRgbaHalf ? 8 : kind == kDstNv12 ? 1 : 2;
+    }
+    uint32_t planes() const { return kind == kDstRgba8 || kind == kDstRgbaHalf ? 1 : 2; }
+    bool hdr() const { return kind == kDstRgbaHalf || kind == kDstP010Pq; }   // the sinks of Hap HDR (BC6H) frames
+};
+
+// The launches of launch_block_decode for the BC kinds: to RGBA8 (bc_decode_kernel; Hap Q Alpha merges its alpha texture) or
+// to NV12 / P010 (bc_decode_yuv_kernel; Hap Q Alpha decodes its YCoCg texture only, alpha is dropped).
 template <int KIND>
-void launch_bc_decode(uint32_t frames, cudaStream_t st, const uint8_t *blocks, const uint8_t *alpha, const BcDecodeGeom &g, uint8_t *rgba,
-                      const uint32_t *frame_results)
+void launch_bc_decode_slice(int dst_kind, const dim3 &grid, cudaStream_t st, const uint8_t *blocks, const uint8_t *alpha,
+                            const BcDecodeGeom &g, const YuvOutGeom &yg, uint8_t *pixels, uint8_t *chroma, const uint32_t *results)
 {
+    if (dst_kind == kDstRgba8)
+        HAP_KLAUNCH(kStBcDecode, bc_decode_kernel<KIND>, grid, dim3(kBcThreads), 0, st, blocks, alpha, g, pixels, results);
+    else if (dst_kind == kDstP010)
+        HAP_KLAUNCH(kStBcDecode, (bc_decode_yuv_kernel<KIND, HapB200YUV_P010>), grid, dim3(kBcThreads), 0, st, blocks, yg, pixels, chroma, results);
+    else
+        HAP_KLAUNCH(kStBcDecode, (bc_decode_yuv_kernel<KIND, HapB200YUV_NV12>), grid, dim3(kBcThreads), 0, st, blocks, yg, pixels, chroma, results);
+}
+
+// Blocks of ci (frame f's at blocks + f*blocks_stride, its second texture, Hap Q Alpha's alpha, second_offset behind them) ->
+// the pictures d (frame f's planes at d's + f*frame_stride, rows `pitch` apart).  The kernel follows ci.bc_kind and the sink:
+// launch_bc_decode_slice for the BC kinds, bc6h_decode_kernel (RGBA16F) or bc6h_decode_yuv_kernel (HDR10 P010) for BC6H.
+// frame_results (optional): HapResult per frame; a frame that failed is written as zeros.  BC6H signedness per frame from
+// frame_formats, or from ci.fmt[0] for every frame without them.  One launch per kBcFramesPerLaunch frames, counted as bc_decode.
+uint32_t launch_block_decode(const CodecInfo &ci, const PictureDst &d, const uint8_t *blocks, uint64_t second_offset, uint32_t frames,
+                             uint64_t blocks_stride, uint32_t width, uint32_t height, uint64_t frame_stride, uint64_t pitch,
+                             const uint32_t *frame_results, const uint32_t *frame_formats, cudaStream_t st)
+{
+    const bool two_planes = d.planes() == 2;
+    const uint16_t *table = nullptr;
+    if (d.kind == kDstP010Pq && !(table = pq_table(d.unit_nits, kPqOut))) return HapResult_Internal_Error;
+    BcDecodeGeom g = BcDecodeGeom();
+    YuvOutGeom yg = YuvOutGeom();
+    if (!two_planes) g = bc_decode_geom(width, height, (uint32_t)pitch, ci.textures == 2, blocks_stride, blocks_stride, frame_stride);
+    else if (d.kind == kDstP010Pq) yg = yuv_out_geom(width, height, (uint32_t)pitch, blocks_stride, frame_stride, yuv_pq_out_coeffs(d.color_space));
+    else yg = yuv_out_geom(width, height, (uint32_t)pitch, blocks_stride, frame_stride, d.kind == kDstP010 ? HapB200YUV_P010 : HapB200YUV_NV12, d.color_space);
+    const unsigned ctas = two_planes ? (unsigned)yuv_out_ctas(yg) : bc_ctas(g.blocks_x, g.blocks_y);   // (pitch < 2^32)
+    const uint32_t is_signed = ci.fmt[0] == HapFmt_RGB_BPTC_SFLOAT ? 1u : 0u;
     for (uint32_t f0 = 0; f0 < frames; f0 += kBcFramesPerLaunch) {
-        const dim3 grid(bc_ctas(g.blocks_x, g.blocks_y), frames - f0 < kBcFramesPerLaunch ? frames - f0 : kBcFramesPerLaunch);
-        HAP_KLAUNCH(kStBcDecode, bc_decode_kernel<KIND>, grid, dim3(kBcThreads), 0, st, blocks + f0 * g.in_stride, alpha + f0 * g.alpha_stride, g,
-                    rgba + f0 * g.frame_bytes, frame_results ? frame_results + f0 : nullptr);
-    }
-}
-
-uint32_t launch_block_decode(const uint8_t *blocks, const uint8_t *alpha, uint32_t frames, uint64_t blocks_stride,
-                             uint64_t alpha_stride, uint32_t width, uint32_t height, const CodecInfo &ci, uint8_t *rgba,
-                             uint64_t frame_stride, uint64_t row_bytes, cudaStream_t st, const uint32_t *frame_results = nullptr)
-{
-    const BcDecodeGeom g = bc_decode_geom(width, height, (uint32_t)row_bytes, ci.textures == 2, blocks_stride, alpha_stride, frame_stride);
-    switch (ci.bc_kind) {
-    case kBcDxt1: launch_bc_decode<kBcDxt1>(frames, st, blocks, alpha, g, rgba, frame_results); break;
-    case kBcDxt5: launch_bc_decode<kBcDxt5>(frames, st, blocks, alpha, g, rgba, frame_results); break;
-    case kBcRgtc1: launch_bc_decode<kBcRgtc1>(frames, st, blocks, alpha, g, rgba, frame_results); break;
-    case kBcYCoCg:
-    case kBcYCoCgPlusAlpha: launch_bc_decode<kBcYCoCg>(frames, st, blocks, alpha, g, rgba, frame_results); break;
-    case kBcBc7: launch_bc_decode<kBcBc7>(frames, st, blocks, alpha, g, rgba, frame_results); break;
-    default: return HapResult_Internal_Error;
-    }
-    return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
-}
-
-// The NV12 / P010 sink of K8 (yuv_sink.cuh): blocks -> luma and chroma planes, frame f's at luma / chroma + f*frame_stride.
-// Launches count as bc_decode.  Hap Q Alpha decodes its YCoCg texture only: alpha is dropped.
-template <int KIND, int LAYOUT>
-void launch_bc_decode_yuv(uint32_t frames, cudaStream_t st, const uint8_t *blocks, const YuvOutGeom &g, uint8_t *luma, uint8_t *chroma,
-                          const uint32_t *frame_results)
-{
-    for (uint32_t f0 = 0; f0 < frames; f0 += kBcFramesPerLaunch) {
-        const dim3 grid((unsigned)yuv_out_ctas(g), frames - f0 < kBcFramesPerLaunch ? frames - f0 : kBcFramesPerLaunch);
-        HAP_KLAUNCH(kStBcDecode, (bc_decode_yuv_kernel<KIND, LAYOUT>), grid, dim3(kBcThreads), 0, st, blocks + f0 * g.in_stride, g,
-                    luma + f0 * g.frame_bytes, chroma + f0 * g.frame_bytes, frame_results ? frame_results + f0 : nullptr);
-    }
-}
-
-template <int KIND>
-void launch_bc_decode_yuv_layout(uint32_t frames, cudaStream_t st, const uint8_t *blocks, const YuvOutGeom &g, uint8_t *luma, uint8_t *chroma,
-                                 unsigned layout, const uint32_t *frame_results)
-{
-    if (layout == HapB200YUV_P010) launch_bc_decode_yuv<KIND, HapB200YUV_P010>(frames, st, blocks, g, luma, chroma, frame_results);
-    else launch_bc_decode_yuv<KIND, HapB200YUV_NV12>(frames, st, blocks, g, luma, chroma, frame_results);
-}
-
-uint32_t launch_block_decode_yuv(const uint8_t *blocks, uint32_t frames, uint64_t blocks_stride, uint32_t width, uint32_t height,
-                                 const CodecInfo &ci, uint8_t *luma, uint8_t *chroma, uint64_t frame_stride, uint64_t pitch, unsigned layout,
-                                 unsigned color_space, cudaStream_t st, const uint32_t *frame_results = nullptr)
-{
-    const YuvOutGeom g = yuv_out_geom(width, height, (uint32_t)pitch, blocks_stride, frame_stride, layout, color_space);   // (pitch < 2^32)
-    switch (ci.bc_kind) {
-    case kBcDxt1: launch_bc_decode_yuv_layout<kBcDxt1>(frames, st, blocks, g, luma, chroma, layout, frame_results); break;
-    case kBcDxt5: launch_bc_decode_yuv_layout<kBcDxt5>(frames, st, blocks, g, luma, chroma, layout, frame_results); break;
-    case kBcRgtc1: launch_bc_decode_yuv_layout<kBcRgtc1>(frames, st, blocks, g, luma, chroma, layout, frame_results); break;
-    case kBcYCoCg:
-    case kBcYCoCgPlusAlpha: launch_bc_decode_yuv_layout<kBcYCoCg>(frames, st, blocks, g, luma, chroma, layout, frame_results); break;
-    case kBcBc7: launch_bc_decode_yuv_layout<kBcBc7>(frames, st, blocks, g, luma, chroma, layout, frame_results); break;
-    default: return HapResult_Internal_Error;
-    }
-    return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
-}
-
-// BC6H (Hap HDR) blocks -> RGBA16F.  Signedness per frame from frame_formats, or is_signed for all.  One launch per
-// kBcFramesPerLaunch frames.
-uint32_t launch_bc6h_decode(const uint8_t *blocks, uint32_t frames, uint64_t blocks_stride, uint32_t width, uint32_t height, uint8_t *rgba,
-                            uint64_t frame_stride, uint64_t row_bytes, cudaStream_t st, const uint32_t *frame_results,
-                            const uint32_t *frame_formats, bool is_signed)
-{
-    const BcDecodeGeom g = bc_decode_geom(width, height, (uint32_t)row_bytes, false, blocks_stride, 0, frame_stride);
-    for (uint32_t f0 = 0; f0 < frames; f0 += kBcFramesPerLaunch) {
-        const dim3 grid(bc_ctas(g.blocks_x, g.blocks_y), frames - f0 < kBcFramesPerLaunch ? frames - f0 : kBcFramesPerLaunch);
-        HAP_KLAUNCH(kStBcDecode, bc6h_decode_kernel, grid, dim3(kBcThreads), 0, st, blocks + f0 * g.in_stride, g, rgba + f0 * g.frame_bytes,
-                    frame_results ? frame_results + f0 : nullptr, frame_formats ? frame_formats + f0 : nullptr, is_signed ? 1u : 0u);
-    }
-    return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
-}
-
-// The HDR10 sink of K8 (yuv_sink.cuh): BC6H blocks -> BT.2020 PQ P010 planes, frame f's at luma / chroma + f*frame_stride.
-// Signedness per frame from frame_formats, or is_signed for all.  Launches count as bc_decode.
-uint32_t launch_bc6h_decode_yuv_pq(const uint8_t *blocks, uint32_t frames, uint64_t blocks_stride, uint32_t width, uint32_t height,
-                                   uint8_t *luma, uint8_t *chroma, uint64_t frame_stride, uint64_t pitch, unsigned color_space,
-                                   unsigned unit_nits, cudaStream_t st, const uint32_t *frame_results, const uint32_t *frame_formats,
-                                   bool is_signed)
-{
-    const uint16_t *table = pq_table(unit_nits, kPqOut);
-    if (!table) return HapResult_Internal_Error;
-    const YuvOutGeom g = yuv_out_geom(width, height, (uint32_t)pitch, blocks_stride, frame_stride, yuv_pq_out_coeffs(color_space));   // (pitch < 2^32)
-    for (uint32_t f0 = 0; f0 < frames; f0 += kBcFramesPerLaunch) {
-        const dim3 grid((unsigned)yuv_out_ctas(g), frames - f0 < kBcFramesPerLaunch ? frames - f0 : kBcFramesPerLaunch);
-        HAP_KLAUNCH(kStBcDecode, bc6h_decode_yuv_kernel, grid, dim3(kBcThreads), 0, st, blocks + f0 * g.in_stride, g, luma + f0 * g.frame_bytes,
-                    chroma + f0 * g.frame_bytes, frame_results ? frame_results + f0 : nullptr, frame_formats ? frame_formats + f0 : nullptr,
-                    is_signed ? 1u : 0u, table);
+        const dim3 grid(ctas, frames - f0 < kBcFramesPerLaunch ? frames - f0 : kBcFramesPerLaunch);
+        const uint8_t *b = blocks + f0 * blocks_stride;
+        uint8_t *pixels = (uint8_t *)d.pixels + f0 * frame_stride, *chroma = two_planes ? (uint8_t *)d.chroma + f0 * frame_stride : nullptr;
+        const uint32_t *res = frame_results ? frame_results + f0 : nullptr, *fmts = frame_formats ? frame_formats + f0 : nullptr;
+        switch (ci.bc_kind) {
+        case kBcDxt1: launch_bc_decode_slice<kBcDxt1>(d.kind, grid, st, b, b + second_offset, g, yg, pixels, chroma, res); break;
+        case kBcDxt5: launch_bc_decode_slice<kBcDxt5>(d.kind, grid, st, b, b + second_offset, g, yg, pixels, chroma, res); break;
+        case kBcRgtc1: launch_bc_decode_slice<kBcRgtc1>(d.kind, grid, st, b, b + second_offset, g, yg, pixels, chroma, res); break;
+        case kBcYCoCg:
+        case kBcYCoCgPlusAlpha: launch_bc_decode_slice<kBcYCoCg>(d.kind, grid, st, b, b + second_offset, g, yg, pixels, chroma, res); break;
+        case kBcBc7: launch_bc_decode_slice<kBcBc7>(d.kind, grid, st, b, b + second_offset, g, yg, pixels, chroma, res); break;
+        case kBcBc6h:
+            if (two_planes)
+                HAP_KLAUNCH(kStBcDecode, bc6h_decode_yuv_kernel, grid, dim3(kBcThreads), 0, st, b, yg, pixels, chroma, res, fmts, is_signed, table);
+            else
+                HAP_KLAUNCH(kStBcDecode, bc6h_decode_kernel, grid, dim3(kBcThreads), 0, st, b, g, pixels, res, fmts, is_signed);
+            break;
+        default: return HapResult_Internal_Error;
+        }
     }
     return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
 }
@@ -866,6 +868,328 @@ void work_function(void *p, unsigned int)
     reinterpret_cast<WorkState *>(p)->claimed.fetch_add(1, std::memory_order_relaxed);
 }
 
+// ---- the picture encoders and decoders behind the picture entry points ---------------------------------------------------
+
+// width x height NV12 (bpp 1) / P010 (bpp 2) planes with one pitch: the chroma plane's rows hold as many bytes as luma's.
+// aligned: the batch entry points' rules besides (16-byte aligned pitch, planes and frame stride).
+bool yuv_geometry_ok(const void *luma, const void *chroma, unsigned width, unsigned height, unsigned long pitch, unsigned long frameStride,
+                     bool aligned, unsigned long bpp)
+{
+    return chroma && rgba_geometry_ok(luma, width, height, pitch, frameStride, aligned, bpp) && (!aligned || (uintptr_t)chroma % 16 == 0);
+}
+
+// A planar picture's four planes (see PictureSrc): luma (and alpha) as rgba_geometry_ok with `pitch`; Cb and Cr of
+// p.chroma_width(width) samples per row, rows p.chroma_pitch apart.  Alpha-only pictures are checked as their alpha plane.
+bool planar_geometry_ok(const PictureSrc &p, unsigned width, unsigned height, unsigned long pitch, unsigned long frameStride, bool aligned)
+{
+    if (!rgba_geometry_ok(p.pixels, width, height, pitch, frameStride, aligned, p.sample_bytes())) return false;
+    if (p.alpha_only) return true;
+    if (!p.chroma || !p.cr || p.chroma_pitch < p.sample_bytes() * p.chroma_width(width) || p.chroma_pitch > HAPB200_MAX_ROW_BYTES) return false;
+    return !aligned || (((uintptr_t)p.chroma | (uintptr_t)p.cr | (uintptr_t)p.alpha | p.chroma_pitch) % 16 == 0);
+}
+
+bool picture_geometry_ok(const PictureSrc &p, unsigned width, unsigned height, unsigned long pitch, unsigned long frameStride, bool aligned)
+{
+    if (is_planar_src(p.kind)) return planar_geometry_ok(p, width, height, pitch, frameStride, aligned);
+    if (p.planes() == 1) return rgba_geometry_ok(p.pixels, width, height, pitch, frameStride, aligned, p.sample_bytes());
+    return yuv_geometry_ok(p.pixels, p.chroma, width, height, pitch, frameStride, aligned, p.sample_bytes());
+}
+
+bool picture_geometry_ok(const PictureDst &d, unsigned width, unsigned height, unsigned long pitch, unsigned long frameStride, bool aligned)
+{
+    if (d.planes() == 1) return rgba_geometry_ok(d.pixels, width, height, pitch, frameStride, aligned, d.sample_bytes());
+    return yuv_geometry_ok(d.pixels, d.chroma, width, height, pitch, frameStride, aligned, d.sample_bytes());
+}
+
+// The picture encoders of every codec with a block compressor and of Hap HDR, behind the codec-taking RGBA8 entry points (which
+// refuse Hap7), the BC7 ones (which ask for it by name), the YUV, planar, RGBA16F and HDR10 ones
+unsigned block_encode_picture_batch(const CodecInfo &ci, const PictureSrc &p, unsigned frames, unsigned long frameStride, unsigned width,
+                                    unsigned height, unsigned long pitch, void *blocks, unsigned long blocksStride, void *stream)
+{
+    if (!blocks || frames == 0 || !picture_geometry_ok(p, width, height, pitch, frameStride, true) || ((uintptr_t)blocks | blocksStride) % 16)
+        return HapResult_Bad_Arguments;
+    HAP_ENTER(p.pixels, blocks);
+    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
+        return launch_block_encode(ci, p, frames, frameStride, width, height, pitch, (uint8_t *)blocks, blocksStride,
+                                   texture_bytes(width, height, ci, 0), st);
+    });
+}
+
+unsigned encode_picture_batch(const CodecInfo &ci, const PictureSrc &p, unsigned frames, unsigned long frameStride, unsigned width,
+                              unsigned height, unsigned long pitch, unsigned compressor, unsigned chunkCount, void *out,
+                              unsigned long outStride, unsigned long long *used, void *stream)
+{
+    if (!out || !used || frames == 0 || chunkCount == 0 || !picture_geometry_ok(p, width, height, pitch, frameStride, true) ||
+        (compressor != HapCompressorNone && compressor != HapCompressorSnappy))
+        return HapResult_Bad_Arguments;
+    if (outStride < max_encoded_length_rgba(width, height, ci, chunkCount)) return HapResult_Buffer_Too_Small;
+    HAP_ENTER(p.pixels, out);
+    // Hap Q from RGBA8 without the chroma refinement, Snappy: the fused encoder (hapq_fused.cuh) when the chunks allow it
+    const FusedPictures fp = {(const uint8_t *)p.pixels, bc_encode_geom(width, height, (uint32_t)pitch, frameStride, 0, 0)};
+    const bool fuse = HAPB200_FUSED_HAPQ && ci.bc_kind == kBcYCoCg && p.kind == kSrcRgba8 && g_chroma_refine.load() == 0 &&
+                      compressor == HapCompressorSnappy;
+    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
+        const uint64_t t[2] = {texture_bytes(width, height, ci, 0), texture_bytes(width, height, ci, 1)};
+        return encode_frames_from_blocks(
+            frames, ci.textures, t, ci.fmt, compressor, chunkCount, (uint8_t *)out, outStride, used, st,
+            [&](uint8_t *tex, uint64_t stride) {
+                return launch_block_encode(ci, p, frames, frameStride, width, height, pitch, tex, stride, align16(t[0]), st);
+            },
+            fuse ? &fp : nullptr);
+    });
+}
+
+// One picture in host or device memory, its arguments checked: its planes are copied into tight device scratch (rows
+// align16(row bytes) apart, chroma after luma; planar pictures: Cb, Cr and alpha after luma) and encoded as a batch of one by
+// encode_picture_batch.  cap: the frame's size bound.
+unsigned encode_picture(const CodecInfo &ci, const PictureSrc &p, unsigned width, unsigned height, unsigned long pitch, unsigned compressor,
+                        unsigned chunkCount, void *outputBuffer, unsigned long outputBufferBytes, unsigned long *outputBufferBytesUsed)
+{
+    if (!outputBuffer || !outputBufferBytesUsed || chunkCount == 0 || !picture_geometry_ok(p, width, height, pitch, 0, false) ||
+        (compressor != HapCompressorNone && compressor != HapCompressorSnappy))
+        return HapResult_Bad_Arguments;
+    const unsigned long cap = max_encoded_length_rgba(width, height, ci, chunkCount);
+    if (outputBufferBytes < cap) return HapResult_Buffer_Too_Small;
+    HAP_ENTER(p.pixels, outputBuffer);
+    CallStream call(!is_device(p.pixels) && !is_device(p.chroma) && !is_device(p.cr) && !is_device(p.alpha) && !is_device(outputBuffer));
+    cudaStream_t st = call.st;
+    DevBuf img(st), frame(st), used(st);
+    const uint64_t row = p.sample_bytes() * width, tight = align16(row);   // (RGBA8, RGBA16F: tight = row, width is a multiple of 4)
+    // the planes to copy: {source, its pitch, row bytes, rows, tight pitch, where the device copy's pointer goes}
+    struct Plane { const void *from; uint64_t pitch, row, rows, tight; const void **to; };
+    PictureSrc dev = p;
+    Plane planes[4];
+    int n = 0;
+    if (is_planar_src(p.kind)) {
+        const uint64_t crow = p.sample_bytes() * (p.alpha_only ? 0 : p.chroma_width(width)), ctight = align16(crow);
+        dev.chroma_pitch = ctight;
+        if (p.alpha_only) {
+            planes[n++] = {p.alpha, pitch, row, height, tight, &dev.alpha};
+        } else {
+            planes[n++] = {p.pixels, pitch, row, height, tight, &dev.pixels};
+            planes[n++] = {p.chroma, p.chroma_pitch, crow, p.chroma_height(height), ctight, &dev.chroma};
+            planes[n++] = {p.cr, p.chroma_pitch, crow, p.chroma_height(height), ctight, &dev.cr};
+            if (p.alpha) planes[n++] = {p.alpha, pitch, row, height, tight, &dev.alpha};
+        }
+    } else {
+        planes[n++] = {p.pixels, pitch, row, height, tight, &dev.pixels};
+        if (p.planes() == 2) planes[n++] = {p.chroma, pitch, row, height / 2, tight, &dev.chroma};
+    }
+    uint64_t plane_bytes = 0;
+    for (int i = 0; i < n; i++) plane_bytes += planes[i].tight * planes[i].rows;
+    if (!img.alloc(plane_bytes) || !frame.alloc(align16(cap)) || !used.alloc(32)) { cudaGetLastError(); return HapResult_Internal_Error; }
+    uint64_t at = 0;
+    for (int i = 0; i < n; i++) {
+        const Plane &q = planes[i];
+        *q.to = img.as<uint8_t>() + at;
+        if (cudaMemcpy2DAsync(img.as<uint8_t>() + at, q.tight, q.from, q.pitch, q.row, q.rows, cudaMemcpyDefault, st) != cudaSuccess) {
+            cudaGetLastError();
+            return HapResult_Internal_Error;
+        }
+        at += q.tight * q.rows;
+    }
+    if (dev.alpha_only) dev.pixels = dev.chroma = dev.cr = dev.alpha;
+    uint32_t r = encode_picture_batch(ci, dev, 1, align16(plane_bytes), width, height, tight, compressor, chunkCount, frame.p, align16(cap),
+                                      used.as<unsigned long long>(), st);
+    if (r != HapResult_No_Error) return r;
+    unsigned long long total = 0;
+    if (cudaMemcpyAsync(&total, used.p, sizeof total, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess ||
+        total > outputBufferBytes || cudaMemcpyAsync(outputBuffer, frame.p, total, cudaMemcpyDefault, st) != cudaSuccess ||
+        cudaStreamSynchronize(st) != cudaSuccess) { cudaGetLastError(); return HapResult_Internal_Error; }
+    *outputBufferBytesUsed = (unsigned long)total;
+    return HapResult_No_Error;
+}
+
+// ---- the families' own arguments and pictures ----
+
+CodecInfo bc7_codec()
+{
+    CodecInfo ci;
+    codec_info(HapB200Codec_Hap7, ci);
+    return ci;
+}
+
+// the codecs the YUV encoders take (every one with a block compressor that encodes colour) and the layouts and colour spaces
+bool yuv_args_ok(unsigned layout, unsigned colorSpace, unsigned codec, CodecInfo &ci)
+{
+    return layout <= HapB200YUV_P010 && colorSpace <= HapB200YUV_BT709_Full && codec_info(codec, ci) && codec_encodes(ci) && ci.bc_kind != kBcRgtc1;
+}
+
+PictureSrc yuv_picture(const void *luma, const void *chroma, unsigned layout, unsigned colorSpace)
+{
+    return {layout == HapB200YUV_P010 ? kSrcP010 : kSrcNv12, luma, chroma, colorSpace};
+}
+
+// the codecs (every one with a block compressor; HapA only with an alpha plane), subsamplings, depths and colour spaces the
+// planar encoders take
+bool planar_args_ok(const void *alpha, unsigned subsampling, unsigned bitDepth, unsigned colorSpace, unsigned codec, CodecInfo &ci)
+{
+    return subsampling <= HapB200Chroma_444 && (bitDepth == 8 || bitDepth == 10 || bitDepth == 12) && colorSpace <= HapB200YUV_BT709_Full &&
+           codec_info(codec, ci) && codec_encodes(ci) && (ci.bc_kind != kBcRgtc1 || alpha);
+}
+
+// Hap1 and HapY do not read alpha; HapA reads alpha alone (the picture's other planes are the alpha plane, never read)
+PictureSrc planar_picture(const CodecInfo &ci, const void *luma, const void *cb, const void *cr, const void *alpha, unsigned long chromaPitch,
+                          unsigned subsampling, unsigned bitDepth, unsigned colorSpace)
+{
+    PictureSrc p{planar_src(subsampling, bitDepth > 8), luma, cb, colorSpace};
+    p.cr = cr;
+    p.alpha = ci.bc_kind == kBcDxt1 || ci.bc_kind == kBcYCoCg ? nullptr : alpha;
+    p.chroma_pitch = chromaPitch;
+    p.bit_depth = bitDepth;
+    if (ci.bc_kind == kBcRgtc1) {
+        p.alpha_only = true;
+        p.pixels = p.chroma = p.cr = alpha;
+    }
+    return p;
+}
+
+// HapB200YUV_BT2020_Limited or _Full, and a unitNits of 1 .. 10000 cd/m2
+bool yuv_pq_args_ok(unsigned colorSpace, unsigned unitNits)
+{
+    return (colorSpace == HapB200YUV_BT2020_Limited || colorSpace == HapB200YUV_BT2020_Full) && unitNits >= 1 && unitNits <= 10000;
+}
+
+PictureSrc yuv_pq_picture(const void *luma, const void *chroma, unsigned colorSpace, unsigned unitNits)
+{
+    return {kSrcP010Pq, luma, chroma, colorSpace, unitNits};
+}
+
+// the layouts and colour spaces the YUV decoders take (BT.601 / BT.709; no BT.2020)
+bool yuv_out_args_ok(unsigned layout, unsigned colorSpace) { return layout <= HapB200YUV_P010 && colorSpace <= HapB200YUV_BT709_Full; }
+
+PictureDst yuv_out_picture(void *luma, void *chroma, unsigned layout, unsigned colorSpace)
+{
+    return {layout == HapB200YUV_P010 ? kDstP010 : kDstNv12, luma, chroma, colorSpace};
+}
+
+// the Hap HDR batch decoders' codec: each frame's signedness comes from its own texture format (frame_formats)
+CodecInfo hap_hdr_batch_codec()
+{
+    CodecInfo ci;
+    bc6h_codec(HapFmt_RGB_BPTC_UFLOAT, ci);
+    return ci;
+}
+
+// ---- decoding ----
+
+// The blocks of every frame (frame f's at blocks + f*blocksStride, Hap Q Alpha's alpha texture texture_bytes(.., 0) behind
+// them) -> the pictures d, frameStride apart
+unsigned block_decode_picture_batch(const CodecInfo &ci, const PictureDst &d, const void *blocks, unsigned frames, unsigned long blocksStride,
+                                    unsigned width, unsigned height, unsigned long frameStride, unsigned long pitch, void *stream)
+{
+    if (!blocks || frames == 0 || !picture_geometry_ok(d, width, height, pitch, frameStride, true) || ((uintptr_t)blocks | blocksStride) % 16)
+        return HapResult_Bad_Arguments;
+    HAP_ENTER(blocks, d.pixels);
+    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
+        return launch_block_decode(ci, d, (const uint8_t *)blocks, texture_bytes(width, height, ci, 0), frames, blocksStride, width, height,
+                                   frameStride, pitch, nullptr, nullptr, st);
+    });
+}
+
+// The texture half of the picture batch decoders: every texture of every frame decoded into device scratch `tex` (frame f at
+// f * (align16(t[0]) + align16(t[1])), texture 1 at align16(t[0]) inside it) and texture 0's format into `formats`, both
+// allocated here, and results[f] set as the batch decoders report it.  The decoded size must equal the texture size: each
+// texture is offered exactly that much room per frame (the slot stride is wider: both textures of a frame share a slot, so a
+// texture that over-declares its size must not reach its neighbour or the next frame's slot).  Then a frame whose textures are
+// not ci's reports Bad_Frame (Hap HDR: hap_check_bc6h_frames_kernel, which takes either signedness; the others:
+// hap_check_texture_kernel per texture), other failures keep the decoder's code.
+uint32_t decode_textures_batch(const CodecInfo &ci, const void *in, unsigned frames, unsigned long inStride, const unsigned long long *inBytes,
+                               unsigned maxChunks, const uint64_t t[2], DevBuf &tex, DevBuf &formats, unsigned *results, cudaStream_t st)
+{
+    const bool bc6h = ci.bc_kind == kBcBc6h;
+    const uint64_t stride = align16(t[0]) + align16(t[1]);
+    DevBuf used(st), res1(st);
+    if (!tex.alloc(stride * frames + 16) || !used.alloc(8ull * frames) || !formats.alloc(4ull * frames) || (!bc6h && !res1.alloc(4ull * frames))) {
+        cudaGetLastError();
+        return HapResult_Internal_Error;
+    }
+    for (uint32_t ti = 0; ti < ci.textures; ti++) {
+        uint32_t *res = ti == 0 ? results : res1.as<uint32_t>();
+        const uint32_t r = launch_decode_batch((const uint8_t *)in, frames, inStride, inBytes, ti, maxChunks, tex.as<uint8_t>() + (ti ? align16(t[0]) : 0),
+                                               stride, t[ti], used.as<unsigned long long>(), formats.as<uint32_t>(), res, st);
+        if (r != HapResult_No_Error) return r;
+        if (bc6h)
+            HAP_KLAUNCH(kStCollect, hap_check_bc6h_frames_kernel, dim3((frames + 127) / 128), dim3(128), 0, st, (const uint8_t *)in,
+                        (uint64_t)inStride, inBytes, frames, used.as<unsigned long long>(), formats.as<uint32_t>(), (unsigned long long)t[0], results);
+        else
+            HAP_KLAUNCH(kStCollect, hap_check_texture_kernel, dim3((frames + 127) / 128), dim3(128), 0, st, frames, used.as<unsigned long long>(),
+                        formats.as<uint32_t>(), res, (unsigned long long)t[ti], ci.fmt[ti], results);
+    }
+    return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
+}
+
+unsigned decode_picture_batch(const CodecInfo &ci, const PictureDst &d, const void *in, unsigned frames, unsigned long inStride,
+                              const unsigned long long *inBytes, unsigned maxChunks, unsigned width, unsigned height, unsigned long frameStride,
+                              unsigned long pitch, unsigned *results, void *stream)
+{
+    if (!in || !inBytes || !results || frames == 0 || maxChunks == 0 || !picture_geometry_ok(d, width, height, pitch, frameStride, true))
+        return HapResult_Bad_Arguments;
+    HAP_ENTER(in, d.pixels);
+    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
+        const uint64_t t[2] = {texture_bytes(width, height, ci, 0), texture_bytes(width, height, ci, 1)};
+        DevBuf tex(st), formats(st);
+        const uint32_t r = decode_textures_batch(ci, in, frames, inStride, inBytes, maxChunks, t, tex, formats, results, st);
+        if (r != HapResult_No_Error) return r;
+        return launch_block_decode(ci, d, tex.as<uint8_t>(), align16(t[0]), frames, align16(t[0]) + align16(t[1]), width, height, frameStride,
+                                   pitch, results, formats.as<uint32_t>(), st);
+    });
+}
+
+// One frame in host or device memory -> the picture d.  The frame's codec comes from its headers: Hap HDR frames decode to the
+// RGBA16F and HDR10 sinks only, the other flavours to the others (Bad_Frame otherwise).  Its textures, t[i] bytes each, are
+// decoded by HapDecode into device scratch (a texture that does not fill its room: Bad_Frame; the HDR sinks answer Bad_Frame
+// for one too large for it as well, the others what HapDecode answers); then launch_block_decode writes a tight picture (rows
+// sample_bytes * width apart, the chroma plane's height / 2 rows behind luma's), which is copied to the caller's planes.
+uint32_t decode_picture(const PictureDst &d, const void *inputBuffer, unsigned long inputBufferBytes, unsigned width, unsigned height,
+                        unsigned long pitch)
+{
+    if (!inputBuffer || !picture_geometry_ok(d, width, height, pitch, 0, false)) return HapResult_Bad_Arguments;
+    unsigned count = 0, f0 = 0, f1 = 0;
+    uint32_t r = HapGetFrameTextureCount(inputBuffer, inputBufferBytes, &count);
+    if (r != HapResult_No_Error) return r;
+    r = HapGetFrameTextureFormat(inputBuffer, inputBufferBytes, 0, &f0);
+    if (r != HapResult_No_Error) return r;
+    CodecInfo ci;
+    if (d.hdr()) {
+        if (count != 1 || !bc6h_codec(f0, ci)) return HapResult_Bad_Frame;
+    } else {
+        if (count == 2 && (r = HapGetFrameTextureFormat(inputBuffer, inputBufferBytes, 1, &f1)) != HapResult_No_Error) return r;
+        unsigned codec = 0;
+        while (codec_info(codec, ci) && (ci.textures != count || ci.fmt[0] != f0 || (count == 2 && ci.fmt[1] != f1))) codec++;
+        if (!codec_info(codec, ci)) return HapResult_Bad_Frame;
+    }
+    HAP_ENTER(inputBuffer, d.pixels, d.chroma);
+    const uint64_t t[2] = {texture_bytes(width, height, ci, 0), texture_bytes(width, height, ci, 1)};
+    const uint64_t tight = d.sample_bytes() * width, first = tight * height, second = d.planes() == 2 ? tight * (height / 2) : 0;
+    // scratch from the device's stream-ordered pool on the legacy stream (the nested HapDecode calls below write it on
+    // that stream, or on a pooled stream they synchronise before returning): no cudaMalloc/cudaFree, no device-wide sync
+    DevBuf texb(kLegacyStream), imgb(kLegacyStream);
+    if (!texb.alloc(align16(t[0]) + align16(t[1]) + 16) || !imgb.alloc(first + second)) { cudaGetLastError(); return HapResult_Internal_Error; }
+    if (cudaStreamSynchronize(kLegacyStream) != cudaSuccess) { cudaGetLastError(); return HapResult_Internal_Error; }   // the allocations are real now
+    auto serial = [](HapDecodeWorkFunction fn, void *p, unsigned n, void *) { for (unsigned i = 0; i < n; i++) fn(p, i); };
+    for (unsigned i = 0; i < ci.textures && r == HapResult_No_Error; i++) {
+        unsigned long used = 0;
+        unsigned fmt = 0;
+        r = HapDecode(inputBuffer, inputBufferBytes, i, serial, nullptr, texb.as<uint8_t>() + (i ? align16(t[0]) : 0), t[i], &used, &fmt);
+        if (r == HapResult_No_Error && used != t[i]) r = HapResult_Bad_Frame;
+    }
+    // the room offered is the picture's texture size: to the HDR sinks, a texture too large for it (HapDecode: Buffer_Too_Small)
+    // is not this picture's texture either
+    if (r != HapResult_No_Error) return d.hdr() && r == HapResult_Buffer_Too_Small ? (uint32_t)HapResult_Bad_Frame : r;
+    CallStream call(false);  // the scratch buffers are device memory filled on the legacy stream by HapDecode above
+    cudaStream_t st = call.st;
+    PictureDst img = d;
+    img.pixels = imgb.p;
+    img.chroma = d.planes() == 2 ? imgb.as<uint8_t>() + first : nullptr;
+    r = launch_block_decode(ci, img, texb.as<uint8_t>(), align16(t[0]), 1, 0, width, height, 0, tight, nullptr, nullptr, st);
+    if (r == HapResult_No_Error &&
+        (cudaMemcpy2DAsync(d.pixels, pitch, imgb.p, tight, tight, height, cudaMemcpyDefault, st) != cudaSuccess ||
+         (second && cudaMemcpy2DAsync(d.chroma, pitch, imgb.as<uint8_t>() + first, tight, tight, height / 2, cudaMemcpyDefault, st) != cudaSuccess) ||
+         cudaStreamSynchronize(st) != cudaSuccess)) { cudaGetLastError(); r = HapResult_Internal_Error; }
+    return r;
+}
+
 }  // namespace
 
 // ---- delivery rings: helpers ----
@@ -891,44 +1215,6 @@ __global__ void ring_wait_kernel(const unsigned int *flag, unsigned int value, u
     }
 }
 }  // namespace
-
-// The single-frame picture decoders (HapB200DecodeRGBA, HapB200DecodeRGBAHalf, HapB200DecodeYUV, HapB200DecodeYUVPQ): textures
-// 0 .. count-1 of the frame, t[i] bytes each, are decoded by HapDecode into device scratch (a texture that does not fill its room: Bad_Frame);
-// then launch(textures, picture, tight row bytes, stream) writes a tight picture of bpp bytes per pixel, which is copied to the
-// caller's rows.  With a `chroma` plane the picture has a second plane of height/2 rows of the same width, which launch writes
-// at picture + tight * height and which is copied to chroma's rows (rowBytes apart, as the first plane's).
-template <class Launch>
-uint32_t decode_frame_to_picture(const void *inputBuffer, unsigned long inputBufferBytes, unsigned count, const uint64_t t[2],
-                                 unsigned width, unsigned height, uint64_t bpp, void *picture, unsigned long rowBytes, Launch &&launch,
-                                 void *chroma = nullptr)
-{
-    HAP_ENTER(inputBuffer, picture, chroma);
-    const uint64_t tight = bpp * width, first = tight * height, second = chroma ? tight * (height / 2) : 0;
-    // scratch from the device's stream-ordered pool on the legacy stream (the nested HapDecode calls below write it on
-    // that stream, or on a pooled stream they synchronise before returning): no cudaMalloc/cudaFree, no device-wide sync
-    DevBuf texb(kLegacyStream), imgb(kLegacyStream);
-    if (!texb.alloc(align16(t[0]) + align16(t[1]) + 16) || !imgb.alloc(first + second)) { cudaGetLastError(); return HapResult_Internal_Error; }
-    if (cudaStreamSynchronize(kLegacyStream) != cudaSuccess) { cudaGetLastError(); return HapResult_Internal_Error; }   // the allocations are real now
-    auto serial = [](HapDecodeWorkFunction fn, void *p, unsigned n, void *) { for (unsigned i = 0; i < n; i++) fn(p, i); };
-    uint32_t r = HapResult_No_Error;
-    for (unsigned i = 0; i < count && r == HapResult_No_Error; i++) {
-        unsigned long used = 0;
-        unsigned fmt = 0;
-        r = HapDecode(inputBuffer, inputBufferBytes, i, serial, nullptr, texb.as<uint8_t>() + (i ? align16(t[0]) : 0), t[i], &used, &fmt);
-        if (r == HapResult_No_Error && used != t[i]) r = HapResult_Bad_Frame;
-    }
-    if (r == HapResult_No_Error) {
-        CallStream call(false);  // the scratch buffers are device memory filled on the legacy stream by HapDecode above
-        cudaStream_t st = call.st;
-        r = launch((const uint8_t *)texb.p, imgb.as<uint8_t>(), tight, st);
-        if (r == HapResult_No_Error &&
-            (cudaMemcpy2DAsync(picture, rowBytes, imgb.p, tight, tight, height, cudaMemcpyDefault, st) != cudaSuccess ||
-             (chroma && cudaMemcpy2DAsync(chroma, rowBytes, imgb.as<uint8_t>() + first, tight, tight, height / 2, cudaMemcpyDefault, st) != cudaSuccess) ||
-             cudaStreamSynchronize(st) != cudaSuccess)) { cudaGetLastError(); r = HapResult_Internal_Error; }
-    }
-    return r;
-}
-
 
 // =====================================================================================================
 extern "C" {
@@ -1388,20 +1674,6 @@ unsigned int HapDecode(const void *inputBuffer, unsigned long inputBufferBytes, 
 
 // ---- extensions ----------------------------------------------------------------------------------
 
-static unsigned long texture_bytes(unsigned width, unsigned height, const CodecInfo &ci, unsigned index)
-{
-    if (index >= ci.textures || width % 4 || height % 4) return 0;
-    return (unsigned long)(width / 4) * (height / 4) * ci.block_bytes[index];
-}
-
-static unsigned long max_encoded_length_rgba(unsigned width, unsigned height, const CodecInfo &ci, unsigned chunkCount)
-{
-    unsigned long lens[2] = {texture_bytes(width, height, ci, 0), texture_bytes(width, height, ci, 1)};
-    unsigned fmts[2] = {ci.fmt[0], ci.fmt[1]}, chunks[2] = {chunkCount, chunkCount};
-    if (lens[0] == 0) return 0;
-    return HapMaxEncodedLength(ci.textures, lens, fmts, chunks);
-}
-
 unsigned long HapB200TextureBytes(unsigned int width, unsigned int height, unsigned int codec, unsigned int index)
 {
     CodecInfo ci;
@@ -1414,145 +1686,6 @@ unsigned long HapB200MaxEncodedLengthRGBA(unsigned int width, unsigned int heigh
     CodecInfo ci;
     if (!codec_info(codec, ci)) return 0;
     return max_encoded_length_rgba(width, height, ci, chunkCount);
-}
-
-// width x height NV12 (bpp 1) / P010 (bpp 2) planes with one pitch: the chroma plane's rows hold as many bytes as luma's.
-// aligned: the batch entry points' rules besides (16-byte aligned pitch, planes and frame stride).
-bool yuv_geometry_ok(const void *luma, const void *chroma, unsigned width, unsigned height, unsigned long pitch, unsigned long frameStride,
-                     bool aligned, unsigned long bpp)
-{
-    return chroma && rgba_geometry_ok(luma, width, height, pitch, frameStride, aligned, bpp) && (!aligned || (uintptr_t)chroma % 16 == 0);
-}
-
-// A planar picture's four planes (see PictureSrc): luma (and alpha) as rgba_geometry_ok with `pitch`; Cb and Cr of
-// p.chroma_width(width) samples per row, rows p.chroma_pitch apart.  Alpha-only pictures are checked as their alpha plane.
-bool planar_geometry_ok(const PictureSrc &p, unsigned width, unsigned height, unsigned long pitch, unsigned long frameStride, bool aligned)
-{
-    if (!rgba_geometry_ok(p.pixels, width, height, pitch, frameStride, aligned, p.sample_bytes())) return false;
-    if (p.alpha_only) return true;
-    if (!p.chroma || !p.cr || p.chroma_pitch < p.sample_bytes() * p.chroma_width(width) || p.chroma_pitch > HAPB200_MAX_ROW_BYTES) return false;
-    return !aligned || (((uintptr_t)p.chroma | (uintptr_t)p.cr | (uintptr_t)p.alpha | p.chroma_pitch) % 16 == 0);
-}
-
-bool picture_geometry_ok(const PictureSrc &p, unsigned width, unsigned height, unsigned long pitch, unsigned long frameStride, bool aligned)
-{
-    if (is_planar_src(p.kind)) return planar_geometry_ok(p, width, height, pitch, frameStride, aligned);
-    if (p.planes() == 1) return rgba_geometry_ok(p.pixels, width, height, pitch, frameStride, aligned, p.sample_bytes());
-    return yuv_geometry_ok(p.pixels, p.chroma, width, height, pitch, frameStride, aligned, p.sample_bytes());
-}
-
-// The picture encoders of every codec with a block compressor, behind the codec-taking RGBA8 entry points (which refuse
-// Hap7), the BC7 ones (which ask for it by name) and the YUV ones
-static unsigned block_encode_picture_batch(const CodecInfo &ci, const PictureSrc &p, unsigned frames, unsigned long frameStride,
-                                           unsigned width, unsigned height, unsigned long pitch, void *blocks, unsigned long blocksStride,
-                                           void *stream)
-{
-    if (!blocks || frames == 0 || !picture_geometry_ok(p, width, height, pitch, frameStride, true) || ((uintptr_t)blocks | blocksStride) % 16)
-        return HapResult_Bad_Arguments;
-    HAP_ENTER(p.pixels, blocks);
-    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
-        return launch_block_encode((const uint8_t *)p.pixels, frames, frameStride, width, height, pitch, ci, (uint8_t *)blocks, blocksStride,
-                                   texture_bytes(width, height, ci, 0), st, p.kind, p.yuv(), p.planar());
-    });
-}
-
-static unsigned encode_picture_batch(const CodecInfo &ci, const PictureSrc &p, unsigned frames, unsigned long frameStride, unsigned width,
-                                     unsigned height, unsigned long pitch, unsigned compressor, unsigned chunkCount, void *out,
-                                     unsigned long outStride, unsigned long long *used, void *stream)
-{
-    if (!out || !used || frames == 0 || chunkCount == 0 || !picture_geometry_ok(p, width, height, pitch, frameStride, true) ||
-        (compressor != HapCompressorNone && compressor != HapCompressorSnappy))
-        return HapResult_Bad_Arguments;
-    if (outStride < max_encoded_length_rgba(width, height, ci, chunkCount)) return HapResult_Buffer_Too_Small;
-    HAP_ENTER(p.pixels, out);
-    // Hap Q from RGBA8 without the chroma refinement, Snappy: the fused encoder (hapq_fused.cuh) when the chunks allow it
-    const FusedPictures fp = {(const uint8_t *)p.pixels, bc_encode_geom(width, height, (uint32_t)pitch, frameStride, 0, 0)};
-    const bool fuse = HAPB200_FUSED_HAPQ && ci.bc_kind == kBcYCoCg && p.kind == kSrcRgba8 && g_chroma_refine.load() == 0 &&
-                      compressor == HapCompressorSnappy;
-    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
-        const uint64_t t[2] = {texture_bytes(width, height, ci, 0), texture_bytes(width, height, ci, 1)};
-        return encode_frames_from_blocks(
-            frames, ci.textures, t, ci.fmt, compressor, chunkCount, (uint8_t *)out, outStride, used, st,
-            [&](uint8_t *tex, uint64_t stride) {
-                return launch_block_encode((const uint8_t *)p.pixels, frames, frameStride, width, height, pitch, ci, tex, stride, align16(t[0]),
-                                           st, p.kind, p.yuv(), p.planar());
-            },
-            fuse ? &fp : nullptr);
-    });
-}
-
-// One picture in host or device memory, its arguments checked: its planes are copied into tight device scratch (rows
-// align16(row bytes) apart, chroma after luma; planar pictures: Cb, Cr and alpha after luma) and encoded as a batch of one by
-// batch(device picture, its frame stride, its pitch, out, outStride, used, stream).  cap: the frame's size bound.
-extern "C++" {   // (a template, inside the C ABI block)
-template <class Batch>
-static unsigned encode_one_picture(const PictureSrc &p, unsigned width, unsigned height, unsigned long pitch, unsigned long cap,
-                                   void *outputBuffer, unsigned long outputBufferBytes, unsigned long *outputBufferBytesUsed, Batch &&batch)
-{
-    HAP_ENTER(p.pixels, outputBuffer);
-    CallStream call(!is_device(p.pixels) && !is_device(p.chroma) && !is_device(p.cr) && !is_device(p.alpha) && !is_device(outputBuffer));
-    cudaStream_t st = call.st;
-    DevBuf img(st), frame(st), used(st);
-    const uint64_t row = p.sample_bytes() * width, tight = align16(row);   // (RGBA8, RGBA16F: tight = row, width is a multiple of 4)
-    // the planes to copy: {source, its pitch, row bytes, rows, tight pitch, where the device copy's pointer goes}
-    struct Plane { const void *from; uint64_t pitch, row, rows, tight; const void **to; };
-    PictureSrc dev = p;
-    Plane planes[4];
-    int n = 0;
-    if (is_planar_src(p.kind)) {
-        const uint64_t crow = p.sample_bytes() * (p.alpha_only ? 0 : p.chroma_width(width)), ctight = align16(crow);
-        dev.chroma_pitch = ctight;
-        if (p.alpha_only) {
-            planes[n++] = {p.alpha, pitch, row, height, tight, &dev.alpha};
-        } else {
-            planes[n++] = {p.pixels, pitch, row, height, tight, &dev.pixels};
-            planes[n++] = {p.chroma, p.chroma_pitch, crow, p.chroma_height(height), ctight, &dev.chroma};
-            planes[n++] = {p.cr, p.chroma_pitch, crow, p.chroma_height(height), ctight, &dev.cr};
-            if (p.alpha) planes[n++] = {p.alpha, pitch, row, height, tight, &dev.alpha};
-        }
-    } else {
-        planes[n++] = {p.pixels, pitch, row, height, tight, &dev.pixels};
-        if (p.planes() == 2) planes[n++] = {p.chroma, pitch, row, height / 2, tight, &dev.chroma};
-    }
-    uint64_t plane_bytes = 0;
-    for (int i = 0; i < n; i++) plane_bytes += planes[i].tight * planes[i].rows;
-    if (!img.alloc(plane_bytes) || !frame.alloc(align16(cap)) || !used.alloc(32)) { cudaGetLastError(); return HapResult_Internal_Error; }
-    uint64_t at = 0;
-    for (int i = 0; i < n; i++) {
-        const Plane &q = planes[i];
-        *q.to = img.as<uint8_t>() + at;
-        if (cudaMemcpy2DAsync(img.as<uint8_t>() + at, q.tight, q.from, q.pitch, q.row, q.rows, cudaMemcpyDefault, st) != cudaSuccess) {
-            cudaGetLastError();
-            return HapResult_Internal_Error;
-        }
-        at += q.tight * q.rows;
-    }
-    if (dev.alpha_only) dev.pixels = dev.chroma = dev.cr = dev.alpha;
-    uint32_t r = batch(dev, align16(plane_bytes), tight, frame.p, align16(cap), used.as<unsigned long long>(), st);
-    if (r != HapResult_No_Error) return r;
-    unsigned long long total = 0;
-    if (cudaMemcpyAsync(&total, used.p, sizeof total, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess ||
-        total > outputBufferBytes || cudaMemcpyAsync(outputBuffer, frame.p, total, cudaMemcpyDefault, st) != cudaSuccess ||
-        cudaStreamSynchronize(st) != cudaSuccess) { cudaGetLastError(); return HapResult_Internal_Error; }
-    *outputBufferBytesUsed = (unsigned long)total;
-    return HapResult_No_Error;
-}
-}  // extern "C++"
-
-static unsigned encode_picture(const CodecInfo &ci, const PictureSrc &p, unsigned width, unsigned height, unsigned long pitch, unsigned compressor,
-                               unsigned chunkCount, void *outputBuffer, unsigned long outputBufferBytes, unsigned long *outputBufferBytesUsed)
-{
-    if (!outputBuffer || !outputBufferBytesUsed || chunkCount == 0 || !picture_geometry_ok(p, width, height, pitch, 0, false) ||
-        (compressor != HapCompressorNone && compressor != HapCompressorSnappy))
-        return HapResult_Bad_Arguments;
-    const unsigned long cap = max_encoded_length_rgba(width, height, ci, chunkCount);
-    if (outputBufferBytes < cap) return HapResult_Buffer_Too_Small;
-    return encode_one_picture(p, width, height, pitch, cap, outputBuffer, outputBufferBytes, outputBufferBytesUsed,
-                              [&](const PictureSrc &dev, uint64_t fstride, uint64_t tight, void *out, uint64_t ostride, unsigned long long *used,
-                                  cudaStream_t st) {
-                                  return encode_picture_batch(ci, dev, 1, fstride, width, height, tight, compressor, chunkCount, out, ostride,
-                                                              used, st);
-                              });
 }
 
 unsigned int HapB200BlockEncodeBatch(const void *rgba, unsigned int frames, unsigned long frameStride, unsigned int width,
@@ -1569,15 +1702,9 @@ unsigned int HapB200BlockDecodeBatch(const void *blocks, unsigned int frames, un
                                      unsigned long rowBytes, void *stream)
 {
     CodecInfo ci;
-    if (!blocks || frames == 0 || !codec_info(codec, ci) || !rgba_geometry_ok(rgba, width, height, rowBytes, frameStride, true) ||
-        ((uintptr_t)blocks | blocksStride) % 16)
-        return HapResult_Bad_Arguments;
-    HAP_ENTER(blocks, rgba);
-    const uint8_t *b = (const uint8_t *)blocks;
-    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
-        return launch_block_decode(b, b + HapB200TextureBytes(width, height, codec, 0), frames, blocksStride, blocksStride, width, height, ci,
-                                   (uint8_t *)rgba, frameStride, rowBytes, st);
-    });
+    if (!codec_info(codec, ci)) return HapResult_Bad_Arguments;
+    return block_decode_picture_batch(ci, {kDstRgba8, rgba, nullptr, 0}, blocks, frames, blocksStride, width, height, frameStride, rowBytes,
+                                      stream);
 }
 
 unsigned int HapB200EncodeBatch(unsigned int count, const void **textures, unsigned long *textureStrides,
@@ -1629,13 +1756,6 @@ unsigned int HapB200EncodeRGBA(const void *rgba, unsigned int width, unsigned in
 
 // ---- Hap R encoding: RGBA8 -> BC7 (bc7_encode.cuh), the RGBA8 encoders' plumbing with the Hap7 codec -------------------
 
-static CodecInfo bc7_codec()
-{
-    CodecInfo ci;
-    codec_info(HapB200Codec_Hap7, ci);
-    return ci;
-}
-
 unsigned int HapB200EncodeRGBABC7(const void *rgba, unsigned int width, unsigned int height, unsigned long rowBytes,
                                   unsigned int compressor, unsigned int chunkCount, void *outputBuffer,
                                   unsigned long outputBufferBytes, unsigned long *outputBufferBytesUsed)
@@ -1658,17 +1778,6 @@ unsigned int HapB200BlockEncodeBC7Batch(const void *rgba, unsigned int frames, u
 }
 
 // ---- NV12 / P010 -> Hap, Hap Alpha, Hap Q, Hap Q Alpha: the picture encoders with a YUV source (yuv_source.cuh) ----------
-
-// the codecs the YUV encoders take (every one with a block compressor that encodes colour) and the layouts and colour spaces
-static bool yuv_args_ok(unsigned layout, unsigned colorSpace, unsigned codec, CodecInfo &ci)
-{
-    return layout <= HapB200YUV_P010 && colorSpace <= HapB200YUV_BT709_Full && codec_info(codec, ci) && codec_encodes(ci) && ci.bc_kind != kBcRgtc1;
-}
-
-static PictureSrc yuv_picture(const void *luma, const void *chroma, unsigned layout, unsigned colorSpace)
-{
-    return {layout == HapB200YUV_P010 ? kSrcP010 : kSrcNv12, luma, chroma, colorSpace};
-}
 
 unsigned int HapB200EncodeYUV(const void *luma, const void *chroma, unsigned int width, unsigned int height, unsigned long pitch,
                               unsigned int layout, unsigned int colorSpace, unsigned int codec, unsigned int compressor,
@@ -1703,30 +1812,6 @@ unsigned int HapB200BlockEncodeYUVBatch(const void *luma, const void *chroma, un
 
 // ---- planar Y'CbCr 4:2:0 / 4:2:2 / 4:4:4 (+ alpha) -> Hap, Hap Alpha, Hap Q, Hap Q Alpha, Hap Alpha-Only: the picture
 // encoders with a planar source (yuv_source.cuh) ----------------------------------------------------------------------------
-
-// the codecs (every one with a block compressor; HapA only with an alpha plane), subsamplings, depths and colour spaces the
-// planar encoders take
-static bool planar_args_ok(const void *alpha, unsigned subsampling, unsigned bitDepth, unsigned colorSpace, unsigned codec, CodecInfo &ci)
-{
-    return subsampling <= HapB200Chroma_444 && (bitDepth == 8 || bitDepth == 10 || bitDepth == 12) && colorSpace <= HapB200YUV_BT709_Full &&
-           codec_info(codec, ci) && codec_encodes(ci) && (ci.bc_kind != kBcRgtc1 || alpha);
-}
-
-// Hap1 and HapY do not read alpha; HapA reads alpha alone (the picture's other planes are the alpha plane, never read)
-static PictureSrc planar_picture(const CodecInfo &ci, const void *luma, const void *cb, const void *cr, const void *alpha,
-                                 unsigned long chromaPitch, unsigned subsampling, unsigned bitDepth, unsigned colorSpace)
-{
-    PictureSrc p{planar_src(subsampling, bitDepth > 8), luma, cb, colorSpace};
-    p.cr = cr;
-    p.alpha = ci.bc_kind == kBcDxt1 || ci.bc_kind == kBcYCoCg ? nullptr : alpha;
-    p.chroma_pitch = chromaPitch;
-    p.bit_depth = bitDepth;
-    if (ci.bc_kind == kBcRgtc1) {
-        p.alpha_only = true;
-        p.pixels = p.chroma = p.cr = alpha;
-    }
-    return p;
-}
 
 unsigned int HapB200EncodePlanar(const void *luma, const void *cb, const void *cr, const void *alpha, unsigned int width, unsigned int height,
                                  unsigned long lumaPitch, unsigned long chromaPitch, unsigned int subsampling, unsigned int bitDepth,
@@ -1775,104 +1860,32 @@ unsigned int HapB200DecodeBatch(const void *in, unsigned int frames, unsigned lo
     });
 }
 
-// The texture half of the picture batch decoders (HapB200DecodeRGBABatch, HapB200DecodeYUVBatch): every texture of every frame
-// decoded into device scratch `dxt`, allocated here (frame f at f * (align16(t[0]) + align16(t[1])), texture 1 at align16(t[0])
-// inside it), and results[f] set as HapB200DecodeRGBABatch reports it.
-static uint32_t decode_textures_batch(const void *in, unsigned frames, unsigned long inStride, const unsigned long long *inBytes,
-                                      unsigned maxChunks, const CodecInfo &ci, const uint64_t t[2], DevBuf &dxt, unsigned *results,
-                                      cudaStream_t st)
-{
-    const uint64_t dxt_stride = align16(t[0]) + align16(t[1]);
-    DevBuf used(st), formats(st), res1(st);
-    if (!dxt.alloc(dxt_stride * frames + 16) || !used.alloc(8ull * frames) || !formats.alloc(4ull * frames) || !res1.alloc(4ull * frames)) {
-        cudaGetLastError();
-        return HapResult_Internal_Error;
-    }
-    for (uint32_t ti = 0; ti < ci.textures; ti++) {
-        uint32_t *res = ti == 0 ? results : res1.as<uint32_t>();
-        // the decoded size must equal the texture size: offer exactly that much room per frame (the slot stride is
-        // wider: both textures of a frame share a slot, so a texture that over-declares its size must not reach its
-        // neighbour or the next frame's slot)
-        const uint32_t r = launch_decode_batch((const uint8_t *)in, frames, inStride, inBytes, ti, maxChunks, dxt.as<uint8_t>() + (ti ? align16(t[0]) : 0),
-                                               dxt_stride, t[ti], used.as<unsigned long long>(), formats.as<uint32_t>(), res, st);
-        if (r != HapResult_No_Error) return r;
-        HAP_KLAUNCH(kStCollect, hap_check_texture_kernel, dim3((frames + 127) / 128), dim3(128), 0, st, frames, used.as<unsigned long long>(),
-                    formats.as<uint32_t>(), res, (unsigned long long)t[ti], ci.fmt[ti], results);
-    }
-    return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
-}
-
 unsigned int HapB200DecodeRGBABatch(const void *in, unsigned int frames, unsigned long inStride, const unsigned long long *inBytes,
                                     unsigned int maxChunks, unsigned int codec, unsigned int width, unsigned int height, void *rgba,
                                     unsigned long frameStride, unsigned long rowBytes, unsigned int *results, void *stream)
 {
     CodecInfo ci;
-    if (!in || !inBytes || !results || frames == 0 || maxChunks == 0 || !codec_info(codec, ci) ||
-        !rgba_geometry_ok(rgba, width, height, rowBytes, frameStride, true))
-        return HapResult_Bad_Arguments;
-    HAP_ENTER(in, rgba);
-    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
-        const uint64_t t[2] = {texture_bytes(width, height, ci, 0), texture_bytes(width, height, ci, 1)};
-        DevBuf dxt(st);
-        const uint32_t r = decode_textures_batch(in, frames, inStride, inBytes, maxChunks, ci, t, dxt, results, st);
-        if (r != HapResult_No_Error) return r;
-        return launch_block_decode(dxt.as<uint8_t>(), dxt.as<uint8_t>() + align16(t[0]), frames, align16(t[0]) + align16(t[1]),
-                                   align16(t[0]) + align16(t[1]), width, height, ci, (uint8_t *)rgba, frameStride, rowBytes, st, results);
-    });
-}
-
-// The codec whose textures a frame has (BC6H frames, Hap HDR, decode to half floats: HapB200DecodeRGBAHalf; Bad_Frame here),
-// for the single-frame RGBA8 and YUV decoders
-static uint32_t frame_codec(const void *inputBuffer, unsigned long inputBufferBytes, CodecInfo &ci)
-{
-    unsigned count = 0, f0 = 0, f1 = 0;
-    uint32_t r = HapGetFrameTextureCount(inputBuffer, inputBufferBytes, &count);
-    if (r != HapResult_No_Error) return r;
-    r = HapGetFrameTextureFormat(inputBuffer, inputBufferBytes, 0, &f0);
-    if (r != HapResult_No_Error) return r;
-    if (count == 2) {
-        r = HapGetFrameTextureFormat(inputBuffer, inputBufferBytes, 1, &f1);
-        if (r != HapResult_No_Error) return r;
-    }
-    unsigned codec = 0;
-    while (codec_info(codec, ci) && (ci.textures != count || ci.fmt[0] != f0 || (count == 2 && ci.fmt[1] != f1))) codec++;
-    return codec_info(codec, ci) ? HapResult_No_Error : HapResult_Bad_Frame;
+    if (!codec_info(codec, ci)) return HapResult_Bad_Arguments;
+    return decode_picture_batch(ci, {kDstRgba8, rgba, nullptr, 0}, in, frames, inStride, inBytes, maxChunks, width, height, frameStride, rowBytes,
+                                results, stream);
 }
 
 unsigned int HapB200DecodeRGBA(const void *inputBuffer, unsigned long inputBufferBytes, unsigned int width, unsigned int height,
                                void *rgba, unsigned long rowBytes)
 {
-    if (!inputBuffer || !rgba_geometry_ok(rgba, width, height, rowBytes, 0, false)) return HapResult_Bad_Arguments;
-    CodecInfo ci;
-    const uint32_t r = frame_codec(inputBuffer, inputBufferBytes, ci);
-    if (r != HapResult_No_Error) return r;
-    const uint64_t t[2] = {texture_bytes(width, height, ci, 0), texture_bytes(width, height, ci, 1)};
-    return decode_frame_to_picture(inputBuffer, inputBufferBytes, ci.textures, t, width, height, 4, rgba, rowBytes,
-                                   [&](const uint8_t *tex, uint8_t *img, uint64_t tight, cudaStream_t st) {
-                                       return launch_block_decode(tex, tex + align16(t[0]), 1, 0, 0, width, height, ci, img, 0, tight, st);
-                                   });
+    return decode_picture({kDstRgba8, rgba, nullptr, 0}, inputBuffer, inputBufferBytes, width, height, rowBytes);
 }
 
 // ---- Hap, Hap Alpha, Hap Q, Hap Q Alpha, Hap Alpha-Only, Hap R -> NV12 / P010: K8 with a YUV sink (yuv_sink.cuh) ----------
-
-// the layouts and colour spaces the YUV decoders take (BT.601 / BT.709; no BT.2020)
-static bool yuv_out_args_ok(unsigned layout, unsigned colorSpace) { return layout <= HapB200YUV_P010 && colorSpace <= HapB200YUV_BT709_Full; }
-
-static uint64_t yuv_sample_bytes(unsigned layout) { return layout == HapB200YUV_P010 ? 2 : 1; }
 
 unsigned int HapB200BlockDecodeYUVBatch(const void *blocks, unsigned int frames, unsigned long blocksStride, unsigned int width,
                                         unsigned int height, unsigned int codec, void *luma, void *chroma, unsigned long frameStride,
                                         unsigned long pitch, unsigned int layout, unsigned int colorSpace, void *stream)
 {
     CodecInfo ci;
-    if (!blocks || frames == 0 || !codec_info(codec, ci) || !yuv_out_args_ok(layout, colorSpace) ||
-        !yuv_geometry_ok(luma, chroma, width, height, pitch, frameStride, true, yuv_sample_bytes(layout)) || ((uintptr_t)blocks | blocksStride) % 16)
-        return HapResult_Bad_Arguments;
-    HAP_ENTER(blocks, luma);
-    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
-        return launch_block_decode_yuv((const uint8_t *)blocks, frames, blocksStride, width, height, ci, (uint8_t *)luma, (uint8_t *)chroma,
-                                       frameStride, pitch, layout, colorSpace, st);
-    });
+    if (!codec_info(codec, ci) || !yuv_out_args_ok(layout, colorSpace)) return HapResult_Bad_Arguments;
+    return block_decode_picture_batch(ci, yuv_out_picture(luma, chroma, layout, colorSpace), blocks, frames, blocksStride, width, height,
+                                      frameStride, pitch, stream);
 }
 
 unsigned int HapB200DecodeYUVBatch(const void *in, unsigned int frames, unsigned long inStride, const unsigned long long *inBytes,
@@ -1881,236 +1894,87 @@ unsigned int HapB200DecodeYUVBatch(const void *in, unsigned int frames, unsigned
                                    unsigned int *results, void *stream)
 {
     CodecInfo ci;
-    if (!in || !inBytes || !results || frames == 0 || maxChunks == 0 || !codec_info(codec, ci) || !yuv_out_args_ok(layout, colorSpace) ||
-        !yuv_geometry_ok(luma, chroma, width, height, pitch, frameStride, true, yuv_sample_bytes(layout)))
-        return HapResult_Bad_Arguments;
-    HAP_ENTER(in, luma);
-    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
-        const uint64_t t[2] = {texture_bytes(width, height, ci, 0), texture_bytes(width, height, ci, 1)};
-        DevBuf dxt(st);
-        const uint32_t r = decode_textures_batch(in, frames, inStride, inBytes, maxChunks, ci, t, dxt, results, st);
-        if (r != HapResult_No_Error) return r;
-        return launch_block_decode_yuv(dxt.as<uint8_t>(), frames, align16(t[0]) + align16(t[1]), width, height, ci, (uint8_t *)luma,
-                                       (uint8_t *)chroma, frameStride, pitch, layout, colorSpace, st, results);
-    });
+    if (!codec_info(codec, ci) || !yuv_out_args_ok(layout, colorSpace)) return HapResult_Bad_Arguments;
+    return decode_picture_batch(ci, yuv_out_picture(luma, chroma, layout, colorSpace), in, frames, inStride, inBytes, maxChunks, width, height,
+                                frameStride, pitch, results, stream);
 }
 
 unsigned int HapB200DecodeYUV(const void *inputBuffer, unsigned long inputBufferBytes, unsigned int width, unsigned int height, void *luma,
                               void *chroma, unsigned long pitch, unsigned int layout, unsigned int colorSpace)
 {
-    if (!inputBuffer || !yuv_out_args_ok(layout, colorSpace) ||
-        !yuv_geometry_ok(luma, chroma, width, height, pitch, 0, false, yuv_sample_bytes(layout)))
-        return HapResult_Bad_Arguments;
-    CodecInfo ci;
-    const uint32_t r = frame_codec(inputBuffer, inputBufferBytes, ci);
-    if (r != HapResult_No_Error) return r;
-    const uint64_t t[2] = {texture_bytes(width, height, ci, 0), texture_bytes(width, height, ci, 1)};
-    return decode_frame_to_picture(
-        inputBuffer, inputBufferBytes, ci.textures, t, width, height, yuv_sample_bytes(layout), luma, pitch,
-        [&](const uint8_t *tex, uint8_t *img, uint64_t tight, cudaStream_t st) {
-            return launch_block_decode_yuv(tex, 1, 0, width, height, ci, img, img + tight * height, 0, tight, layout, colorSpace, st);
-        },
-        chroma);
+    if (!yuv_out_args_ok(layout, colorSpace)) return HapResult_Bad_Arguments;
+    return decode_picture(yuv_out_picture(luma, chroma, layout, colorSpace), inputBuffer, inputBufferBytes, width, height, pitch);
 }
 
-bool is_bc6h_format(unsigned f) { return f == HapFmt_RGB_BPTC_UFLOAT || f == HapFmt_RGB_BPTC_SFLOAT; }
+// ---- Hap HDR -> RGBA16F: BC6H (bc6h_decode.cuh) ----
 
 unsigned int HapB200BlockDecodeHalfBatch(const void *blocks, unsigned int frames, unsigned long blocksStride, unsigned int width,
                                          unsigned int height, unsigned int textureFormat, void *rgbaHalf, unsigned long frameStride,
                                          unsigned long rowBytes, void *stream)
 {
-    if (!blocks || frames == 0 || !is_bc6h_format(textureFormat) || !rgba_geometry_ok(rgbaHalf, width, height, rowBytes, frameStride, true, 8) ||
-        ((uintptr_t)blocks | blocksStride) % 16)
-        return HapResult_Bad_Arguments;
-    HAP_ENTER(blocks, rgbaHalf);
-    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
-        return launch_bc6h_decode((const uint8_t *)blocks, frames, blocksStride, width, height, (uint8_t *)rgbaHalf, frameStride, rowBytes, st,
-                                  nullptr, nullptr, textureFormat == HapFmt_RGB_BPTC_SFLOAT);
-    });
-}
-
-// the bytes of the one BC6H texture of a width x height Hap HDR frame
-static uint64_t bc6h_texture_bytes(unsigned width, unsigned height) { return (uint64_t)(width / 4) * (height / 4) * 16; }
-
-// The texture half of the Hap HDR batch decoders (HapB200DecodeRGBAHalfBatch, HapB200DecodeYUVPQBatch): texture 0 of every
-// frame decoded into device scratch `tex` (frame f at f * align16(bc6h_texture_bytes)) and its format into `formats`, both
-// allocated here, and results[f] set as HapB200DecodeRGBAHalfBatch reports it.
-static uint32_t decode_bc6h_textures_batch(const void *in, unsigned frames, unsigned long inStride, const unsigned long long *inBytes,
-                                           unsigned maxChunks, unsigned width, unsigned height, DevBuf &tex, DevBuf &formats,
-                                           unsigned *results, cudaStream_t st)
-{
-    const uint64_t t0 = bc6h_texture_bytes(width, height), stride = align16(t0);
-    DevBuf used(st);
-    if (!tex.alloc(stride * frames + 16) || !used.alloc(8ull * frames) || !formats.alloc(4ull * frames)) {
-        cudaGetLastError();
-        return HapResult_Internal_Error;
-    }
-    // texture 0 of every frame, offered exactly its BC6H size; then a frame that is not one BC6H texture of that size
-    // reports Bad_Frame, other failures keep the decoder's code, and failed frames are zeroed
-    const uint32_t r = launch_decode_batch((const uint8_t *)in, frames, inStride, inBytes, 0, maxChunks, tex.as<uint8_t>(), stride, t0,
-                                           used.as<unsigned long long>(), formats.as<uint32_t>(), results, st);
-    if (r != HapResult_No_Error) return r;
-    HAP_KLAUNCH(kStCollect, hap_check_bc6h_frames_kernel, dim3((frames + 127) / 128), dim3(128), 0, st, (const uint8_t *)in, (uint64_t)inStride,
-                inBytes, frames, used.as<unsigned long long>(), formats.as<uint32_t>(), (unsigned long long)t0, results);
-    return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
+    CodecInfo ci;
+    if (!bc6h_codec(textureFormat, ci)) return HapResult_Bad_Arguments;
+    return block_decode_picture_batch(ci, {kDstRgbaHalf, rgbaHalf, nullptr, 0}, blocks, frames, blocksStride, width, height, frameStride,
+                                      rowBytes, stream);
 }
 
 unsigned int HapB200DecodeRGBAHalfBatch(const void *in, unsigned int frames, unsigned long inStride, const unsigned long long *inBytes,
                                         unsigned int maxChunks, unsigned int width, unsigned int height, void *rgbaHalf,
                                         unsigned long frameStride, unsigned long rowBytes, unsigned int *results, void *stream)
 {
-    if (!in || !inBytes || !results || frames == 0 || maxChunks == 0 || !rgba_geometry_ok(rgbaHalf, width, height, rowBytes, frameStride, true, 8))
-        return HapResult_Bad_Arguments;
-    HAP_ENTER(in, rgbaHalf);
-    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
-        DevBuf tex(st), formats(st);
-        const uint32_t r = decode_bc6h_textures_batch(in, frames, inStride, inBytes, maxChunks, width, height, tex, formats, results, st);
-        if (r != HapResult_No_Error) return r;
-        return launch_bc6h_decode(tex.as<uint8_t>(), frames, align16(bc6h_texture_bytes(width, height)), width, height, (uint8_t *)rgbaHalf,
-                                  frameStride, rowBytes, st, results, formats.as<uint32_t>(), false);
-    });
+    return decode_picture_batch(hap_hdr_batch_codec(), {kDstRgbaHalf, rgbaHalf, nullptr, 0}, in, frames, inStride, inBytes, maxChunks, width,
+                                height, frameStride, rowBytes, results, stream);
 }
-
-extern "C++" {
-// The single-frame Hap HDR decoders (HapB200DecodeRGBAHalf, HapB200DecodeYUVPQ): a frame that is not one BC6H texture of the
-// picture's size is Bad_Frame; else decode_frame_to_picture, with launch(texture, picture, tight, stream, is_signed).
-template <class Launch>
-static uint32_t decode_bc6h_frame_to_picture(const void *inputBuffer, unsigned long inputBufferBytes, unsigned width, unsigned height,
-                                             uint64_t bpp, void *picture, unsigned long rowBytes, Launch &&launch, void *chroma = nullptr)
-{
-    unsigned count = 0, fmt = 0;
-    uint32_t r = HapGetFrameTextureCount(inputBuffer, inputBufferBytes, &count);
-    if (r != HapResult_No_Error) return r;
-    r = HapGetFrameTextureFormat(inputBuffer, inputBufferBytes, 0, &fmt);
-    if (r != HapResult_No_Error) return r;
-    if (count != 1 || !is_bc6h_format(fmt)) return HapResult_Bad_Frame;
-    const uint64_t t[2] = {bc6h_texture_bytes(width, height), 0};
-    r = decode_frame_to_picture(
-        inputBuffer, inputBufferBytes, 1, t, width, height, bpp, picture, rowBytes,
-        [&](const uint8_t *tex, uint8_t *img, uint64_t tight, cudaStream_t st) { return launch(tex, img, tight, st, fmt == HapFmt_RGB_BPTC_SFLOAT); },
-        chroma);
-    // the room offered is the picture's texture size: a texture too large for it (HapDecode: Buffer_Too_Small) is not this
-    // picture's texture either
-    return r == HapResult_Buffer_Too_Small ? (uint32_t)HapResult_Bad_Frame : r;
-}
-}  // extern "C++"
 
 unsigned int HapB200DecodeRGBAHalf(const void *inputBuffer, unsigned long inputBufferBytes, unsigned int width, unsigned int height,
                                    void *rgbaHalf, unsigned long rowBytes)
 {
-    if (!inputBuffer || !rgba_geometry_ok(rgbaHalf, width, height, rowBytes, 0, false, 8)) return HapResult_Bad_Arguments;
-    return decode_bc6h_frame_to_picture(inputBuffer, inputBufferBytes, width, height, 8, rgbaHalf, rowBytes,
-                                        [&](const uint8_t *tex, uint8_t *img, uint64_t tight, cudaStream_t st, bool sgn) {
-                                            return launch_bc6h_decode(tex, 1, 0, width, height, img, 0, tight, st, nullptr, nullptr, sgn);
-                                        });
+    return decode_picture({kDstRgbaHalf, rgbaHalf, nullptr, 0}, inputBuffer, inputBufferBytes, width, height, rowBytes);
 }
 
 // ---- Hap HDR encoding: RGBA16F -> BC6H (bc6h_encode.cuh) ----
-
-// HapMaxEncodedLength of the one BC6H texture of a width x height picture
-static unsigned long bc6h_max_encoded_length(unsigned width, unsigned height, unsigned textureFormat, unsigned chunkCount)
-{
-    unsigned long len = (unsigned long)(width / 4) * (height / 4) * 16;
-    unsigned fmt = textureFormat, chunks = chunkCount;
-    return HapMaxEncodedLength(1, &len, &fmt, &chunks);
-}
-
-// The BC6H encoders of an RGBA16F picture (kSrcRgbaHalf) and of an HDR10 P010 picture (kSrcP010Pq)
-static unsigned block_encode_bc6h_batch(const PictureSrc &p, unsigned frames, unsigned long frameStride, unsigned width, unsigned height,
-                                        unsigned long pitch, unsigned textureFormat, void *blocks, unsigned long blocksStride, void *stream)
-{
-    if (!blocks || frames == 0 || !is_bc6h_format(textureFormat) || !picture_geometry_ok(p, width, height, pitch, frameStride, true) ||
-        ((uintptr_t)blocks | blocksStride) % 16)
-        return HapResult_Bad_Arguments;
-    HAP_ENTER(p.pixels, blocks);
-    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
-        return launch_bc6h_encode(p, frames, frameStride, width, height, pitch, (uint8_t *)blocks, blocksStride,
-                                  textureFormat == HapFmt_RGB_BPTC_SFLOAT, st);
-    });
-}
-
-static unsigned encode_bc6h_batch(const PictureSrc &p, unsigned frames, unsigned long frameStride, unsigned width, unsigned height,
-                                  unsigned long pitch, unsigned textureFormat, unsigned compressor, unsigned chunkCount, void *out,
-                                  unsigned long outStride, unsigned long long *used, void *stream)
-{
-    if (!out || !used || frames == 0 || chunkCount == 0 || !is_bc6h_format(textureFormat) ||
-        !picture_geometry_ok(p, width, height, pitch, frameStride, true) || ((uintptr_t)out | outStride) % 16 ||
-        (compressor != HapCompressorNone && compressor != HapCompressorSnappy))
-        return HapResult_Bad_Arguments;
-    if (outStride < bc6h_max_encoded_length(width, height, textureFormat, chunkCount)) return HapResult_Buffer_Too_Small;
-    HAP_ENTER(p.pixels, out);
-    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
-        const uint64_t t[2] = {(uint64_t)(width / 4) * (height / 4) * 16, 0};
-        const uint32_t fmt[2] = {textureFormat, 0};
-        return encode_frames_from_blocks(frames, 1, t, fmt, compressor, chunkCount, (uint8_t *)out, outStride, used, st,
-                                         [&](uint8_t *tex, uint64_t stride) {
-                                             return launch_bc6h_encode(p, frames, frameStride, width, height, pitch, tex, stride,
-                                                                       textureFormat == HapFmt_RGB_BPTC_SFLOAT, st);
-                                         });
-    });
-}
-
-static unsigned encode_bc6h_picture(const PictureSrc &p, unsigned width, unsigned height, unsigned long pitch, unsigned textureFormat,
-                                    unsigned compressor, unsigned chunkCount, void *outputBuffer, unsigned long outputBufferBytes,
-                                    unsigned long *outputBufferBytesUsed)
-{
-    if (!outputBuffer || !outputBufferBytesUsed || chunkCount == 0 || !is_bc6h_format(textureFormat) ||
-        !picture_geometry_ok(p, width, height, pitch, 0, false) || (compressor != HapCompressorNone && compressor != HapCompressorSnappy))
-        return HapResult_Bad_Arguments;
-    const unsigned long cap = bc6h_max_encoded_length(width, height, textureFormat, chunkCount);
-    if (outputBufferBytes < cap) return HapResult_Buffer_Too_Small;
-    return encode_one_picture(p, width, height, pitch, cap, outputBuffer, outputBufferBytes, outputBufferBytesUsed,
-                              [&](const PictureSrc &dev, uint64_t fstride, uint64_t tight, void *out, uint64_t ostride, unsigned long long *used,
-                                  cudaStream_t st) {
-                                  return encode_bc6h_batch(dev, 1, fstride, width, height, tight, textureFormat, compressor, chunkCount, out,
-                                                           ostride, used, st);
-                              });
-}
 
 unsigned int HapB200BlockEncodeHalfBatch(const void *rgbaHalf, unsigned int frames, unsigned long frameStride, unsigned int width,
                                          unsigned int height, unsigned long rowBytes, unsigned int textureFormat, void *blocks,
                                          unsigned long blocksStride, void *stream)
 {
-    return block_encode_bc6h_batch(rgba_half_picture(rgbaHalf), frames, frameStride, width, height, rowBytes, textureFormat, blocks,
-                                   blocksStride, stream);
+    CodecInfo ci;
+    if (!bc6h_codec(textureFormat, ci)) return HapResult_Bad_Arguments;
+    return block_encode_picture_batch(ci, rgba_half_picture(rgbaHalf), frames, frameStride, width, height, rowBytes, blocks, blocksStride,
+                                      stream);
 }
 
+// (the Hap HDR batch encoders alone refuse an `out` or outStride that is not 16-byte aligned)
 unsigned int HapB200EncodeRGBAHalfBatch(const void *rgbaHalf, unsigned int frames, unsigned long frameStride, unsigned int width,
                                         unsigned int height, unsigned long rowBytes, unsigned int textureFormat, unsigned int compressor,
                                         unsigned int chunkCount, void *out, unsigned long outStride, unsigned long long *used, void *stream)
 {
-    return encode_bc6h_batch(rgba_half_picture(rgbaHalf), frames, frameStride, width, height, rowBytes, textureFormat, compressor, chunkCount,
-                             out, outStride, used, stream);
+    CodecInfo ci;
+    if (!bc6h_codec(textureFormat, ci) || ((uintptr_t)out | outStride) % 16) return HapResult_Bad_Arguments;
+    return encode_picture_batch(ci, rgba_half_picture(rgbaHalf), frames, frameStride, width, height, rowBytes, compressor, chunkCount, out,
+                                outStride, used, stream);
 }
 
 unsigned int HapB200EncodeRGBAHalf(const void *rgbaHalf, unsigned int width, unsigned int height, unsigned long rowBytes,
                                    unsigned int textureFormat, unsigned int compressor, unsigned int chunkCount, void *outputBuffer,
                                    unsigned long outputBufferBytes, unsigned long *outputBufferBytesUsed)
 {
-    return encode_bc6h_picture(rgba_half_picture(rgbaHalf), width, height, rowBytes, textureFormat, compressor, chunkCount, outputBuffer,
-                               outputBufferBytes, outputBufferBytesUsed);
+    CodecInfo ci;
+    if (!bc6h_codec(textureFormat, ci)) return HapResult_Bad_Arguments;
+    return encode_picture(ci, rgba_half_picture(rgbaHalf), width, height, rowBytes, compressor, chunkCount, outputBuffer, outputBufferBytes,
+                          outputBufferBytesUsed);
 }
 
-// ---- Hap HDR encoding from HDR10: P010, BT.2020, PQ -> BC6H, the BC6H encoders with the kSrcP010Pq source (yuv_source.cuh) ----
-
-// HapB200YUV_BT2020_Limited or _Full, and a unitNits of 1 .. 10000 cd/m2
-static bool yuv_pq_args_ok(unsigned colorSpace, unsigned unitNits)
-{
-    return (colorSpace == HapB200YUV_BT2020_Limited || colorSpace == HapB200YUV_BT2020_Full) && unitNits >= 1 && unitNits <= 10000;
-}
-
-static PictureSrc yuv_pq_picture(const void *luma, const void *chroma, unsigned colorSpace, unsigned unitNits)
-{
-    return {kSrcP010Pq, luma, chroma, colorSpace, unitNits};
-}
+// ---- Hap HDR encoding from HDR10: P010, BT.2020, PQ -> BC6H, the Hap HDR encoders with the kSrcP010Pq source (yuv_source.cuh) ----
 
 unsigned int HapB200EncodeYUVPQ(const void *luma, const void *chroma, unsigned int width, unsigned int height, unsigned long pitch,
                                 unsigned int colorSpace, unsigned int unitNits, unsigned int textureFormat, unsigned int compressor,
                                 unsigned int chunkCount, void *outputBuffer, unsigned long outputBufferBytes, unsigned long *outputBufferBytesUsed)
 {
-    if (!yuv_pq_args_ok(colorSpace, unitNits)) return HapResult_Bad_Arguments;
-    return encode_bc6h_picture(yuv_pq_picture(luma, chroma, colorSpace, unitNits), width, height, pitch, textureFormat, compressor, chunkCount,
-                               outputBuffer, outputBufferBytes, outputBufferBytesUsed);
+    CodecInfo ci;
+    if (!yuv_pq_args_ok(colorSpace, unitNits) || !bc6h_codec(textureFormat, ci)) return HapResult_Bad_Arguments;
+    return encode_picture(ci, yuv_pq_picture(luma, chroma, colorSpace, unitNits), width, height, pitch, compressor, chunkCount, outputBuffer,
+                          outputBufferBytes, outputBufferBytesUsed);
 }
 
 unsigned int HapB200EncodeYUVPQBatch(const void *luma, const void *chroma, unsigned int frames, unsigned long frameStride, unsigned int width,
@@ -2118,9 +1982,11 @@ unsigned int HapB200EncodeYUVPQBatch(const void *luma, const void *chroma, unsig
                                      unsigned int textureFormat, unsigned int compressor, unsigned int chunkCount, void *out,
                                      unsigned long outStride, unsigned long long *used, void *stream)
 {
-    if (!yuv_pq_args_ok(colorSpace, unitNits)) return HapResult_Bad_Arguments;
-    return encode_bc6h_batch(yuv_pq_picture(luma, chroma, colorSpace, unitNits), frames, frameStride, width, height, pitch, textureFormat,
-                             compressor, chunkCount, out, outStride, used, stream);
+    CodecInfo ci;
+    if (!yuv_pq_args_ok(colorSpace, unitNits) || !bc6h_codec(textureFormat, ci) || ((uintptr_t)out | outStride) % 16)
+        return HapResult_Bad_Arguments;
+    return encode_picture_batch(ci, yuv_pq_picture(luma, chroma, colorSpace, unitNits), frames, frameStride, width, height, pitch, compressor,
+                                chunkCount, out, outStride, used, stream);
 }
 
 unsigned int HapB200BlockEncodeYUVPQBatch(const void *luma, const void *chroma, unsigned int frames, unsigned long frameStride,
@@ -2128,9 +1994,10 @@ unsigned int HapB200BlockEncodeYUVPQBatch(const void *luma, const void *chroma, 
                                           unsigned int unitNits, unsigned int textureFormat, void *blocks, unsigned long blocksStride,
                                           void *stream)
 {
-    if (!yuv_pq_args_ok(colorSpace, unitNits)) return HapResult_Bad_Arguments;
-    return block_encode_bc6h_batch(yuv_pq_picture(luma, chroma, colorSpace, unitNits), frames, frameStride, width, height, pitch,
-                                   textureFormat, blocks, blocksStride, stream);
+    CodecInfo ci;
+    if (!yuv_pq_args_ok(colorSpace, unitNits) || !bc6h_codec(textureFormat, ci)) return HapResult_Bad_Arguments;
+    return block_encode_picture_batch(ci, yuv_pq_picture(luma, chroma, colorSpace, unitNits), frames, frameStride, width, height, pitch, blocks,
+                                      blocksStride, stream);
 }
 
 // ---- Hap HDR -> HDR10: BC6H -> P010, BT.2020, PQ, K8 with the HDR10 sink (yuv_sink.cuh) ----
@@ -2139,15 +2006,10 @@ unsigned int HapB200BlockDecodeYUVPQBatch(const void *blocks, unsigned int frame
                                           unsigned int height, unsigned int textureFormat, void *luma, void *chroma, unsigned long frameStride,
                                           unsigned long pitch, unsigned int colorSpace, unsigned int unitNits, void *stream)
 {
-    if (!blocks || frames == 0 || !is_bc6h_format(textureFormat) || !yuv_pq_args_ok(colorSpace, unitNits) ||
-        !yuv_geometry_ok(luma, chroma, width, height, pitch, frameStride, true, 2) || ((uintptr_t)blocks | blocksStride) % 16)
-        return HapResult_Bad_Arguments;
-    HAP_ENTER(blocks, luma);
-    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
-        return launch_bc6h_decode_yuv_pq((const uint8_t *)blocks, frames, blocksStride, width, height, (uint8_t *)luma, (uint8_t *)chroma,
-                                         frameStride, pitch, colorSpace, unitNits, st, nullptr, nullptr,
-                                         textureFormat == HapFmt_RGB_BPTC_SFLOAT);
-    });
+    CodecInfo ci;
+    if (!bc6h_codec(textureFormat, ci) || !yuv_pq_args_ok(colorSpace, unitNits)) return HapResult_Bad_Arguments;
+    return block_decode_picture_batch(ci, {kDstP010Pq, luma, chroma, colorSpace, unitNits}, blocks, frames, blocksStride, width, height,
+                                      frameStride, pitch, stream);
 }
 
 unsigned int HapB200DecodeYUVPQBatch(const void *in, unsigned int frames, unsigned long inStride, const unsigned long long *inBytes,
@@ -2155,31 +2017,16 @@ unsigned int HapB200DecodeYUVPQBatch(const void *in, unsigned int frames, unsign
                                      unsigned long frameStride, unsigned long pitch, unsigned int colorSpace, unsigned int unitNits,
                                      unsigned int *results, void *stream)
 {
-    if (!in || !inBytes || !results || frames == 0 || maxChunks == 0 || !yuv_pq_args_ok(colorSpace, unitNits) ||
-        !yuv_geometry_ok(luma, chroma, width, height, pitch, frameStride, true, 2))
-        return HapResult_Bad_Arguments;
-    HAP_ENTER(in, luma);
-    return on_batch_stream(stream, [&](cudaStream_t st) -> uint32_t {
-        DevBuf tex(st), formats(st);
-        const uint32_t r = decode_bc6h_textures_batch(in, frames, inStride, inBytes, maxChunks, width, height, tex, formats, results, st);
-        if (r != HapResult_No_Error) return r;
-        return launch_bc6h_decode_yuv_pq(tex.as<uint8_t>(), frames, align16(bc6h_texture_bytes(width, height)), width, height, (uint8_t *)luma,
-                                         (uint8_t *)chroma, frameStride, pitch, colorSpace, unitNits, st, results, formats.as<uint32_t>(), false);
-    });
+    if (!yuv_pq_args_ok(colorSpace, unitNits)) return HapResult_Bad_Arguments;
+    return decode_picture_batch(hap_hdr_batch_codec(), {kDstP010Pq, luma, chroma, colorSpace, unitNits}, in, frames, inStride, inBytes,
+                                maxChunks, width, height, frameStride, pitch, results, stream);
 }
 
 unsigned int HapB200DecodeYUVPQ(const void *inputBuffer, unsigned long inputBufferBytes, unsigned int width, unsigned int height, void *luma,
                                 void *chroma, unsigned long pitch, unsigned int colorSpace, unsigned int unitNits)
 {
-    if (!inputBuffer || !yuv_pq_args_ok(colorSpace, unitNits) || !yuv_geometry_ok(luma, chroma, width, height, pitch, 0, false, 2))
-        return HapResult_Bad_Arguments;
-    return decode_bc6h_frame_to_picture(
-        inputBuffer, inputBufferBytes, width, height, 2, luma, pitch,
-        [&](const uint8_t *tex, uint8_t *img, uint64_t tight, cudaStream_t st, bool sgn) {
-            return launch_bc6h_decode_yuv_pq(tex, 1, 0, width, height, img, img + tight * height, 0, tight, colorSpace, unitNits, st, nullptr,
-                                             nullptr, sgn);
-        },
-        chroma);
+    if (!yuv_pq_args_ok(colorSpace, unitNits)) return HapResult_Bad_Arguments;
+    return decode_picture({kDstP010Pq, luma, chroma, colorSpace, unitNits}, inputBuffer, inputBufferBytes, width, height, pitch);
 }
 
 // ---- include/hap_mov.h: QuickTime sample tables around Hap frames (host code only) -------------------------

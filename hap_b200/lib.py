@@ -169,32 +169,49 @@ class HapB200(HapABI):
         return int(self.lib.HapB200TextureBytes(w, h, codec, index))
 
     # -- single frame, host or device pointers ------------------------------------------------------
-    def encode_rgba(self, rgba, w, h, codec, compressor=1, chunks=1, row_bytes=None, out=None, out_capacity=None):
-        """rgba: buffer object or (addr, nbytes).  Returns (result, frame bytes | used)."""
+    @staticmethod
+    def _encode_frame(cap, out, encode):
+        """The single-frame encoders' tail: encode(out address, cap, pointer to the bytes used) writes the frame into `out`, or
+        into a new buffer of cap bytes when `out` is None.  Returns (result, frame bytes | used), (result, None) on failure."""
         from .abi import _as_ptr
-        addr, _ = _as_ptr(rgba)
-        cap = self.max_encoded_length_rgba(w, h, codec, chunks) if out_capacity is None else out_capacity
         own = out is None
         if own:
             out = bytearray(max(cap, 1))
         oaddr, _ = _as_ptr(out)
         used = C.c_ulong(0)
-        r = self.lib.HapB200EncodeRGBA(addr, w, h, row_bytes or 4 * w, codec, compressor, chunks, oaddr, cap, C.byref(used))
+        r = encode(oaddr, cap, C.byref(used))
         if r != 0:
             return int(r), None
         return 0, (bytes(memoryview(out)[: used.value]) if own else used.value)
 
-    def decode_rgba(self, frame, w, h, out=None, row_bytes=None, frame_bytes=None):
+    @staticmethod
+    def _decode_frame(frame, frame_bytes, planes, sizes, decode):
+        """The single-frame decoders' tail: decode(frame address, frame bytes, plane addresses...) writes the picture's planes
+        (buffer objects or (addr, nbytes)); when none is given they are allocated here, sizes[i] bytes each.  Returns (result,
+        the planes' bytes when allocated here and the call succeeded -- one plane: its bytes, else a tuple -- else None)."""
         from .abi import _as_ptr
         faddr, fn = _as_ptr(frame)
         if frame_bytes is not None:
             fn = frame_bytes
-        own = out is None
+        own = all(p is None for p in planes)
         if own:
-            out = bytearray(4 * w * h)
-        oaddr, _ = _as_ptr(out)
-        r = self.lib.HapB200DecodeRGBA(faddr, fn, w, h, oaddr, row_bytes or 4 * w)
-        return int(r), (bytes(out) if own and r == 0 else None)
+            planes = [bytearray(n) for n in sizes]
+        r = decode(faddr, fn, *[_as_ptr(p)[0] for p in planes])
+        if not (own and r == 0):
+            return int(r), None
+        return int(r), (bytes(planes[0]) if len(planes) == 1 else tuple(bytes(p) for p in planes))
+
+    def encode_rgba(self, rgba, w, h, codec, compressor=1, chunks=1, row_bytes=None, out=None, out_capacity=None):
+        """rgba: buffer object or (addr, nbytes).  Returns (result, frame bytes | used)."""
+        from .abi import _as_ptr
+        addr, _ = _as_ptr(rgba)
+        cap = self.max_encoded_length_rgba(w, h, codec, chunks) if out_capacity is None else out_capacity
+        return self._encode_frame(cap, out, lambda o, n, used: self.lib.HapB200EncodeRGBA(addr, w, h, row_bytes or 4 * w, codec, compressor,
+                                                                                         chunks, o, n, used))
+
+    def decode_rgba(self, frame, w, h, out=None, row_bytes=None, frame_bytes=None):
+        return self._decode_frame(frame, frame_bytes, [out], [4 * w * h],
+                                  lambda f, n, o: self.lib.HapB200DecodeRGBA(f, n, w, h, o, row_bytes or 4 * w))
 
     # -- device-resident batches (addresses are ints) ---------------------------------------------
     def encode_rgba_batch(self, rgba, frames, frame_stride, w, h, codec, compressor, chunks, out, out_stride, used,
@@ -230,16 +247,8 @@ class HapB200(HapABI):
     # -- Hap HDR (BC6H) -> RGBA16F: 8 bytes per pixel, binary16 R, G, B, A (A = 1.0) ---------------------------------------
     def decode_rgba_half(self, frame, w, h, out=None, row_bytes=None, frame_bytes=None):
         """One Hap HDR frame (buffer object or (addr, nbytes)) -> (result, RGBA16F bytes when `out` is not given)"""
-        from .abi import _as_ptr
-        faddr, fn = _as_ptr(frame)
-        if frame_bytes is not None:
-            fn = frame_bytes
-        own = out is None
-        if own:
-            out = bytearray(8 * w * h)
-        oaddr, _ = _as_ptr(out)
-        r = self.lib.HapB200DecodeRGBAHalf(faddr, fn, w, h, oaddr, row_bytes or 8 * w)
-        return int(r), (bytes(out) if own and r == 0 else None)
+        return self._decode_frame(frame, frame_bytes, [out], [8 * w * h],
+                                  lambda f, n, o: self.lib.HapB200DecodeRGBAHalf(f, n, w, h, o, row_bytes or 8 * w))
 
     def decode_rgba_half_batch(self, frames_ptr, frames, in_stride, in_bytes, max_chunks, w, h, rgba, frame_stride, results,
                                row_bytes=None, stream=None):
@@ -261,15 +270,8 @@ class HapB200(HapABI):
         from .abi import _as_ptr
         addr, _ = _as_ptr(rgba)
         cap = self.max_encoded_length_half(w, h, texture_format, chunks) if out_capacity is None else out_capacity
-        own = out is None
-        if own:
-            out = bytearray(max(cap, 1))
-        oaddr, _ = _as_ptr(out)
-        used = C.c_ulong(0)
-        r = self.lib.HapB200EncodeRGBAHalf(addr, w, h, row_bytes or 8 * w, texture_format, compressor, chunks, oaddr, cap, C.byref(used))
-        if r != 0:
-            return int(r), None
-        return 0, (bytes(memoryview(out)[: used.value]) if own else used.value)
+        return self._encode_frame(cap, out, lambda o, n, used: self.lib.HapB200EncodeRGBAHalf(addr, w, h, row_bytes or 8 * w, texture_format,
+                                                                                             compressor, chunks, o, n, used))
 
     def encode_rgba_half_batch(self, rgba, frames, frame_stride, w, h, texture_format, compressor, chunks, out, out_stride, used,
                                row_bytes=None, stream=None):
@@ -287,15 +289,8 @@ class HapB200(HapABI):
         from .abi import _as_ptr
         addr, _ = _as_ptr(rgba)
         cap = self.max_encoded_length_rgba(w, h, HapB200Codec_Hap7, chunks) if out_capacity is None else out_capacity
-        own = out is None
-        if own:
-            out = bytearray(max(cap, 1))
-        oaddr, _ = _as_ptr(out)
-        used = C.c_ulong(0)
-        r = self.lib.HapB200EncodeRGBABC7(addr, w, h, row_bytes or 4 * w, compressor, chunks, oaddr, cap, C.byref(used))
-        if r != 0:
-            return int(r), None
-        return 0, (bytes(memoryview(out)[: used.value]) if own else used.value)
+        return self._encode_frame(cap, out, lambda o, n, used: self.lib.HapB200EncodeRGBABC7(addr, w, h, row_bytes or 4 * w, compressor, chunks,
+                                                                                            o, n, used))
 
     def encode_rgba_bc7_batch(self, rgba, frames, frame_stride, w, h, compressor, chunks, out, out_stride, used, row_bytes=None,
                               stream=None):
@@ -315,16 +310,9 @@ class HapB200(HapABI):
         laddr, _ = _as_ptr(luma)
         caddr, _ = _as_ptr(chroma)
         cap = self.max_encoded_length_rgba(w, h, codec, chunks) if out_capacity is None else out_capacity
-        own = out is None
-        if own:
-            out = bytearray(max(cap, 1))
-        oaddr, _ = _as_ptr(out)
-        used = C.c_ulong(0)
-        r = self.lib.HapB200EncodeYUV(laddr, caddr, w, h, pitch or (2 if layout == HapB200YUV_P010 else 1) * w, layout, color_space,
-                                      codec, compressor, chunks, oaddr, cap, C.byref(used))
-        if r != 0:
-            return int(r), None
-        return 0, (bytes(memoryview(out)[: used.value]) if own else used.value)
+        return self._encode_frame(cap, out, lambda o, n, used: self.lib.HapB200EncodeYUV(
+            laddr, caddr, w, h, pitch or (2 if layout == HapB200YUV_P010 else 1) * w, layout, color_space, codec, compressor, chunks, o, n,
+            used))
 
     def encode_yuv_batch(self, luma, chroma, frames, frame_stride, w, h, pitch, layout, color_space, codec, compressor, chunks, out,
                          out_stride, used, stream=None):
@@ -354,16 +342,8 @@ class HapB200(HapABI):
         addrs = [0 if b is None else _as_ptr(b)[0] for b in (luma, cb, cr, alpha)]
         lp, cp = self._planar_pitches(w, subsampling, bit_depth, luma_pitch, chroma_pitch)
         cap = self.max_encoded_length_rgba(w, h, codec, chunks) if out_capacity is None else out_capacity
-        own = out is None
-        if own:
-            out = bytearray(max(cap, 1))
-        oaddr, _ = _as_ptr(out)
-        used = C.c_ulong(0)
-        r = self.lib.HapB200EncodePlanar(*addrs, w, h, lp, cp, subsampling, bit_depth, color_space, codec, compressor, chunks, oaddr,
-                                         cap, C.byref(used))
-        if r != 0:
-            return int(r), None
-        return 0, (bytes(memoryview(out)[: used.value]) if own else used.value)
+        return self._encode_frame(cap, out, lambda o, n, used: self.lib.HapB200EncodePlanar(
+            *addrs, w, h, lp, cp, subsampling, bit_depth, color_space, codec, compressor, chunks, o, n, used))
 
     def encode_planar_batch(self, luma, cb, cr, alpha, frames, frame_stride, w, h, luma_pitch, chroma_pitch, subsampling, bit_depth,
                             color_space, codec, compressor, chunks, out, out_stride, used, stream=None):
@@ -381,18 +361,9 @@ class HapB200(HapABI):
     def decode_yuv(self, frame, w, h, layout, color_space, pitch=None, luma=None, chroma=None, frame_bytes=None):
         """frame, luma, chroma: buffer objects or (addr, nbytes).  Returns (result, (luma bytes, chroma bytes)) when it
         allocates the planes (luma and chroma not given), else (result, None)."""
-        from .abi import _as_ptr
-        faddr, fn = _as_ptr(frame)
-        if frame_bytes is not None:
-            fn = frame_bytes
         pitch = pitch or (2 if layout == HapB200YUV_P010 else 1) * w
-        own = luma is None and chroma is None
-        if own:
-            luma, chroma = bytearray(pitch * h), bytearray(pitch * (h // 2))
-        laddr, _ = _as_ptr(luma)
-        caddr, _ = _as_ptr(chroma)
-        r = self.lib.HapB200DecodeYUV(faddr, fn, w, h, laddr, caddr, pitch, layout, color_space)
-        return int(r), ((bytes(luma), bytes(chroma)) if own and r == 0 else None)
+        return self._decode_frame(frame, frame_bytes, [luma, chroma], [pitch * h, pitch * (h // 2)],
+                                  lambda f, n, lu, ch: self.lib.HapB200DecodeYUV(f, n, w, h, lu, ch, pitch, layout, color_space))
 
     def decode_yuv_batch(self, frames_ptr, frames, in_stride, in_bytes, max_chunks, codec, w, h, luma, chroma, frame_stride, pitch, layout,
                          color_space, results, stream=None):
@@ -414,16 +385,8 @@ class HapB200(HapABI):
         laddr, _ = _as_ptr(luma)
         caddr, _ = _as_ptr(chroma)
         cap = self.max_encoded_length_half(w, h, texture_format, chunks) if out_capacity is None else out_capacity
-        own = out is None
-        if own:
-            out = bytearray(max(cap, 1))
-        oaddr, _ = _as_ptr(out)
-        used = C.c_ulong(0)
-        r = self.lib.HapB200EncodeYUVPQ(laddr, caddr, w, h, pitch or 2 * w, color_space, unit_nits, texture_format, compressor, chunks,
-                                        oaddr, cap, C.byref(used))
-        if r != 0:
-            return int(r), None
-        return 0, (bytes(memoryview(out)[: used.value]) if own else used.value)
+        return self._encode_frame(cap, out, lambda o, n, used: self.lib.HapB200EncodeYUVPQ(
+            laddr, caddr, w, h, pitch or 2 * w, color_space, unit_nits, texture_format, compressor, chunks, o, n, used))
 
     def encode_yuv_pq_batch(self, luma, chroma, frames, frame_stride, w, h, pitch, color_space, unit_nits, texture_format, compressor,
                             chunks, out, out_stride, used, stream=None):
@@ -440,18 +403,9 @@ class HapB200(HapABI):
     def decode_yuv_pq(self, frame, w, h, color_space, unit_nits, pitch=None, luma=None, chroma=None, frame_bytes=None):
         """frame, luma, chroma: buffer objects or (addr, nbytes).  Returns (result, (luma bytes, chroma bytes)) when it
         allocates the planes (luma and chroma not given), else (result, None)."""
-        from .abi import _as_ptr
-        faddr, fn = _as_ptr(frame)
-        if frame_bytes is not None:
-            fn = frame_bytes
         pitch = pitch or 2 * w
-        own = luma is None and chroma is None
-        if own:
-            luma, chroma = bytearray(pitch * h), bytearray(pitch * (h // 2))
-        laddr, _ = _as_ptr(luma)
-        caddr, _ = _as_ptr(chroma)
-        r = self.lib.HapB200DecodeYUVPQ(faddr, fn, w, h, laddr, caddr, pitch, color_space, unit_nits)
-        return int(r), ((bytes(luma), bytes(chroma)) if own and r == 0 else None)
+        return self._decode_frame(frame, frame_bytes, [luma, chroma], [pitch * h, pitch * (h // 2)],
+                                  lambda f, n, lu, ch: self.lib.HapB200DecodeYUVPQ(f, n, w, h, lu, ch, pitch, color_space, unit_nits))
 
     def decode_yuv_pq_batch(self, frames_ptr, frames, in_stride, in_bytes, max_chunks, w, h, luma, chroma, frame_stride, pitch, color_space,
                             unit_nits, results, stream=None):

@@ -15,6 +15,7 @@
 #include "hap_mov.h"
 #include "hap_parse.cuh"
 #include "hapq_fused.cuh"
+#include "planar_sink.cuh"
 #include "snappy_decode.cuh"
 #include "snappy_encode.cuh"
 #include "yuv_sink.cuh"
@@ -548,6 +549,7 @@ struct PictureSrc {
         return kind == kSrcRgba8 ? 4 : kind == kSrcRgbaHalf ? 8 : kind == kSrcNv12 ? 1 : 2;
     }
     uint32_t planes() const { return kind == kSrcRgba8 || kind == kSrcRgbaHalf ? 1 : is_planar_src(kind) ? 4 : 2; }
+    bool is_planar() const { return is_planar_src(kind); }
     YuvSrc yuv() const
     {
         return kind == kSrcNv12 || kind == kSrcP010 ? yuv_src(kind - kSrcNv12, color_space, (const uint8_t *)chroma) : YuvSrc();
@@ -649,22 +651,104 @@ uint32_t encode_frames_from_blocks(uint32_t frames, uint32_t count, const uint64
 }
 
 // The picture a decoder writes: an RGBA8 picture (kDstRgba8), an RGBA16F picture (kDstRgbaHalf), the luma and chroma planes of
-// an NV12 / P010 picture (kDstNv12 / kDstP010, yuv_sink.cuh) or of an HDR10 P010 picture (kDstP010Pq, BT.2020 PQ).  The
-// chroma plane's rows are as many bytes apart as luma's.
-enum DstKind { kDstRgba8, kDstRgbaHalf, kDstNv12, kDstP010, kDstP010Pq };
+// an NV12 / P010 picture (kDstNv12 / kDstP010, yuv_sink.cuh) or of an HDR10 P010 picture (kDstP010Pq, BT.2020 PQ), or a planar
+// picture (kDstPlanar*, planar_sink.cuh: one per subsampling and sample width, x8 bytes and x16 16-bit words).  The NV12 / P010
+// chroma plane's rows are as many bytes apart as luma's; rows of the planar chroma planes are chroma_pitch bytes apart, rows of
+// the alpha plane `pitch` bytes apart, as luma's.
+enum DstKind {
+    kDstRgba8, kDstRgbaHalf, kDstNv12, kDstP010, kDstP010Pq,
+    kDstPlanar420x8, kDstPlanar420x16, kDstPlanar422x8, kDstPlanar422x16, kDstPlanar444x8, kDstPlanar444x16
+};
+constexpr bool is_planar_dst(int kind) { return kind >= kDstPlanar420x8 && kind <= kDstPlanar444x16; }
+constexpr int planar_dst(unsigned subsampling, bool wide) { return kDstPlanar420x8 + 2 * (int)subsampling + (wide ? 1 : 0); }
+constexpr int planar_dst_subsampling(int kind) { return (kind - kDstPlanar420x8) / 2; }
+constexpr bool planar_dst_wide(int kind) { return (kind - kDstPlanar420x8) % 2 == 1; }
 struct PictureDst {
     int kind;                 // DstKind
     void *pixels;             // the RGBA8 / RGBA16F picture, or the luma plane
-    void *chroma;             // the interleaved CbCr plane
+    void *chroma;             // the interleaved CbCr plane, or the planar Cb plane
     unsigned color_space;     // HapB200YUVColorSpace
     unsigned unit_nits = 0;   // kDstP010Pq: the luminance of 1.0
+    // kDstPlanar*: the Cr and alpha planes (alpha nullptr: no alpha is written), the chroma planes' pitch and the sample depth.
+    // alpha_only (Hap Alpha-Only): only the alpha plane is written, and pixels, chroma and cr point at it too.
+    void *cr = nullptr, *alpha = nullptr;
+    uint64_t chroma_pitch = 0;
+    unsigned bit_depth = 0;
+    bool alpha_only = false;
     uint64_t sample_bytes() const   // per pixel of a luma / RGBA row
     {
+        if (is_planar_dst(kind)) return planar_dst_wide(kind) ? 2 : 1;
         return kind == kDstRgba8 ? 4 : kind == kDstRgbaHalf ? 8 : kind == kDstNv12 ? 1 : 2;
     }
-    uint32_t planes() const { return kind == kDstRgba8 || kind == kDstRgbaHalf ? 1 : 2; }
+    uint32_t planes() const { return kind == kDstRgba8 || kind == kDstRgbaHalf ? 1 : is_planar_dst(kind) ? 4 : 2; }
+    bool is_planar() const { return is_planar_dst(kind); }
     bool hdr() const { return kind == kDstRgbaHalf || kind == kDstP010Pq; }   // the sinks of Hap HDR (BC6H) frames
+    // the chroma planes' samples per row and rows of a width x height picture
+    uint32_t chroma_width(uint32_t width) const { return planar_dst_subsampling(kind) == HapB200Chroma_444 ? width : width / 2; }
+    uint32_t chroma_height(uint32_t height) const { return planar_dst_subsampling(kind) == HapB200Chroma_420 ? height / 2 : height; }
 };
+
+// The planar sink's launches (planar_sink.cuh): Hap Alpha-Only (kBcRgtc1) writes its alpha plane alone
+// (bc_decode_planar_alpha_kernel), the colour kinds every plane (bc_decode_planar_kernel).
+template <int KIND>
+void launch_planar_decode_slice(int dst_kind, const dim3 &grid, cudaStream_t st, const uint8_t *blocks, const PlanarOut &p, uint8_t *luma,
+                                const uint32_t *results)
+{
+    if constexpr (KIND == kBcRgtc1) {
+        if (planar_dst_wide(dst_kind)) HAP_KLAUNCH(kStBcDecode, bc_decode_planar_alpha_kernel<true>, grid, dim3(kBcThreads), 0, st, blocks, p, results);
+        else HAP_KLAUNCH(kStBcDecode, bc_decode_planar_alpha_kernel<false>, grid, dim3(kBcThreads), 0, st, blocks, p, results);
+    } else {
+#define HAPB200_PLANAR_DECODE(SUB, WIDE) \
+    HAP_KLAUNCH(kStBcDecode, (bc_decode_planar_kernel<KIND, SUB, WIDE>), grid, dim3(kBcThreads), 0, st, blocks, p, luma, results)
+        switch (dst_kind) {
+        case kDstPlanar420x8: HAPB200_PLANAR_DECODE(HapB200Chroma_420, false); break;
+        case kDstPlanar420x16: HAPB200_PLANAR_DECODE(HapB200Chroma_420, true); break;
+        case kDstPlanar422x8: HAPB200_PLANAR_DECODE(HapB200Chroma_422, false); break;
+        case kDstPlanar422x16: HAPB200_PLANAR_DECODE(HapB200Chroma_422, true); break;
+        case kDstPlanar444x8: HAPB200_PLANAR_DECODE(HapB200Chroma_444, false); break;
+        default: HAPB200_PLANAR_DECODE(HapB200Chroma_444, true); break;
+        }
+#undef HAPB200_PLANAR_DECODE
+    }
+}
+
+// launch_block_decode for the planar pictures (its arguments; d.alpha_only exactly when ci is Hap Alpha-Only).  Hap Q Alpha
+// merges its alpha texture, second_offset behind the blocks, when d has an alpha plane.  4:4:4 and Hap Alpha-Only run one
+// thread per block, 4:2:0 and 4:2:2 the warp spans of the NV12 sink.
+uint32_t launch_planar_decode(const CodecInfo &ci, const PictureDst &d, const uint8_t *blocks, uint64_t second_offset, uint32_t frames,
+                              uint64_t blocks_stride, uint32_t width, uint32_t height, uint64_t frame_stride, uint64_t pitch,
+                              const uint32_t *frame_results, cudaStream_t st)
+{
+    if ((ci.bc_kind == kBcRgtc1) != d.alpha_only || ci.bc_kind == kBcBc6h) return HapResult_Bad_Arguments;
+    PlanarOut p;
+    p.g = yuv_out_geom(width, height, (uint32_t)pitch, blocks_stride, frame_stride, planar_out_coeffs(d.bit_depth, d.color_space));
+    p.chroma_pitch = (uint32_t)d.chroma_pitch;   // (planar_geometry_ok: both pitches < 2^32)
+    p.merge_alpha = ci.textures == 2 && d.alpha ? 1u : 0u;
+    p.second_offset = second_offset;
+    const bool per_block = d.alpha_only || planar_dst_subsampling(d.kind) == HapB200Chroma_444;
+    const unsigned ctas = per_block ? bc_ctas(p.g.blocks_x, p.g.blocks_y) : (unsigned)yuv_out_ctas(p.g);
+    for (uint32_t f0 = 0; f0 < frames; f0 += kBcFramesPerLaunch) {
+        const dim3 grid(ctas, frames - f0 < kBcFramesPerLaunch ? frames - f0 : kBcFramesPerLaunch);
+        const uint64_t o = f0 * frame_stride;
+        const uint8_t *b = blocks + f0 * blocks_stride;
+        PlanarOut s = p;
+        s.cb = (uint8_t *)d.chroma + o;
+        s.cr = (uint8_t *)d.cr + o;
+        s.alpha = d.alpha ? (uint8_t *)d.alpha + o : nullptr;
+        uint8_t *luma = (uint8_t *)d.pixels + o;
+        const uint32_t *res = frame_results ? frame_results + f0 : nullptr;
+        switch (ci.bc_kind) {
+        case kBcDxt1: launch_planar_decode_slice<kBcDxt1>(d.kind, grid, st, b, s, luma, res); break;
+        case kBcDxt5: launch_planar_decode_slice<kBcDxt5>(d.kind, grid, st, b, s, luma, res); break;
+        case kBcRgtc1: launch_planar_decode_slice<kBcRgtc1>(d.kind, grid, st, b, s, luma, res); break;
+        case kBcYCoCg:
+        case kBcYCoCgPlusAlpha: launch_planar_decode_slice<kBcYCoCg>(d.kind, grid, st, b, s, luma, res); break;
+        case kBcBc7: launch_planar_decode_slice<kBcBc7>(d.kind, grid, st, b, s, luma, res); break;
+        default: return HapResult_Internal_Error;
+        }
+    }
+    return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
+}
 
 // The launches of launch_block_decode for the BC kinds: to RGBA8 (bc_decode_kernel; Hap Q Alpha merges its alpha texture) or
 // to NV12 / P010 (bc_decode_yuv_kernel; Hap Q Alpha decodes its YCoCg texture only, alpha is dropped).
@@ -682,13 +766,16 @@ void launch_bc_decode_slice(int dst_kind, const dim3 &grid, cudaStream_t st, con
 
 // Blocks of ci (frame f's at blocks + f*blocks_stride, its second texture, Hap Q Alpha's alpha, second_offset behind them) ->
 // the pictures d (frame f's planes at d's + f*frame_stride, rows `pitch` apart).  The kernel follows ci.bc_kind and the sink:
-// launch_bc_decode_slice for the BC kinds, bc6h_decode_kernel (RGBA16F) or bc6h_decode_yuv_kernel (HDR10 P010) for BC6H.
+// launch_bc_decode_slice for the BC kinds, bc6h_decode_kernel (RGBA16F) or bc6h_decode_yuv_kernel (HDR10 P010) for BC6H,
+// launch_planar_decode for the planar pictures.
 // frame_results (optional): HapResult per frame; a frame that failed is written as zeros.  BC6H signedness per frame from
 // frame_formats, or from ci.fmt[0] for every frame without them.  One launch per kBcFramesPerLaunch frames, counted as bc_decode.
 uint32_t launch_block_decode(const CodecInfo &ci, const PictureDst &d, const uint8_t *blocks, uint64_t second_offset, uint32_t frames,
                              uint64_t blocks_stride, uint32_t width, uint32_t height, uint64_t frame_stride, uint64_t pitch,
                              const uint32_t *frame_results, const uint32_t *frame_formats, cudaStream_t st)
 {
+    if (d.is_planar())
+        return launch_planar_decode(ci, d, blocks, second_offset, frames, blocks_stride, width, height, frame_stride, pitch, frame_results, st);
     const bool two_planes = d.planes() == 2;
     const uint16_t *table = nullptr;
     if (d.kind == kDstP010Pq && !(table = pq_table(d.unit_nits, kPqOut))) return HapResult_Internal_Error;
@@ -878,9 +965,11 @@ bool yuv_geometry_ok(const void *luma, const void *chroma, unsigned width, unsig
     return chroma && rgba_geometry_ok(luma, width, height, pitch, frameStride, aligned, bpp) && (!aligned || (uintptr_t)chroma % 16 == 0);
 }
 
-// A planar picture's four planes (see PictureSrc): luma (and alpha) as rgba_geometry_ok with `pitch`; Cb and Cr of
-// p.chroma_width(width) samples per row, rows p.chroma_pitch apart.  Alpha-only pictures are checked as their alpha plane.
-bool planar_geometry_ok(const PictureSrc &p, unsigned width, unsigned height, unsigned long pitch, unsigned long frameStride, bool aligned)
+// A planar picture's four planes (PictureSrc read by the encoders, PictureDst written by the decoders): luma (and alpha) as
+// rgba_geometry_ok with `pitch`; Cb and Cr of p.chroma_width(width) samples per row, rows p.chroma_pitch apart.  Alpha-only
+// pictures are checked as their alpha plane.
+template <class Picture>
+bool planar_geometry_ok(const Picture &p, unsigned width, unsigned height, unsigned long pitch, unsigned long frameStride, bool aligned)
 {
     if (!rgba_geometry_ok(p.pixels, width, height, pitch, frameStride, aligned, p.sample_bytes())) return false;
     if (p.alpha_only) return true;
@@ -897,6 +986,7 @@ bool picture_geometry_ok(const PictureSrc &p, unsigned width, unsigned height, u
 
 bool picture_geometry_ok(const PictureDst &d, unsigned width, unsigned height, unsigned long pitch, unsigned long frameStride, bool aligned)
 {
+    if (d.is_planar()) return planar_geometry_ok(d, width, height, pitch, frameStride, aligned);
     if (d.planes() == 1) return rgba_geometry_ok(d.pixels, width, height, pitch, frameStride, aligned, d.sample_bytes());
     return yuv_geometry_ok(d.pixels, d.chroma, width, height, pitch, frameStride, aligned, d.sample_bytes());
 }
@@ -939,9 +1029,39 @@ unsigned encode_picture_batch(const CodecInfo &ci, const PictureSrc &p, unsigned
     });
 }
 
-// One picture in host or device memory, its arguments checked: its planes are copied into tight device scratch (rows
-// align16(row bytes) apart, chroma after luma; planar pictures: Cb, Cr and alpha after luma) and encoded as a batch of one by
-// encode_picture_batch.  cap: the frame's size bound.
+// The planes the single-frame calls copy between the caller's picture and tight device scratch: the picture's pointer to the
+// plane (field), the caller's pitch, the bytes and rows it holds, and the scratch pitch (align16 of the row bytes).  Luma (or
+// the RGBA picture), then the NV12 / P010 chroma plane, or the planar Cb, Cr and (when given) alpha planes; alpha-only
+// pictures their alpha plane alone.  Returns the count.
+template <class Picture>
+struct PicturePlane {
+    decltype(Picture::pixels) Picture::*field;
+    uint64_t pitch, row, rows, tight;
+};
+template <class Picture>
+int picture_planes(const Picture &p, uint32_t width, uint32_t height, uint64_t pitch, PicturePlane<Picture> planes[4])
+{
+    const uint64_t row = p.sample_bytes() * width, tight = align16(row);   // (RGBA8, RGBA16F: tight = row, width is a multiple of 4)
+    int n = 0;
+    if (p.is_planar()) {
+        const uint64_t crow = p.sample_bytes() * (p.alpha_only ? 0 : p.chroma_width(width)), ctight = align16(crow);
+        if (p.alpha_only) {
+            planes[n++] = {&Picture::alpha, pitch, row, height, tight};
+        } else {
+            planes[n++] = {&Picture::pixels, pitch, row, height, tight};
+            planes[n++] = {&Picture::chroma, p.chroma_pitch, crow, p.chroma_height(height), ctight};
+            planes[n++] = {&Picture::cr, p.chroma_pitch, crow, p.chroma_height(height), ctight};
+            if (p.alpha) planes[n++] = {&Picture::alpha, pitch, row, height, tight};
+        }
+    } else {
+        planes[n++] = {&Picture::pixels, pitch, row, height, tight};
+        if (p.planes() == 2) planes[n++] = {&Picture::chroma, pitch, row, height / 2, tight};
+    }
+    return n;
+}
+
+// One picture in host or device memory, its arguments checked: its planes (picture_planes) are copied into tight device
+// scratch, one behind the other, and encoded as a batch of one by encode_picture_batch.  cap: the frame's size bound.
 unsigned encode_picture(const CodecInfo &ci, const PictureSrc &p, unsigned width, unsigned height, unsigned long pitch, unsigned compressor,
                         unsigned chunkCount, void *outputBuffer, unsigned long outputBufferBytes, unsigned long *outputBufferBytesUsed)
 {
@@ -954,35 +1074,19 @@ unsigned encode_picture(const CodecInfo &ci, const PictureSrc &p, unsigned width
     CallStream call(!is_device(p.pixels) && !is_device(p.chroma) && !is_device(p.cr) && !is_device(p.alpha) && !is_device(outputBuffer));
     cudaStream_t st = call.st;
     DevBuf img(st), frame(st), used(st);
-    const uint64_t row = p.sample_bytes() * width, tight = align16(row);   // (RGBA8, RGBA16F: tight = row, width is a multiple of 4)
-    // the planes to copy: {source, its pitch, row bytes, rows, tight pitch, where the device copy's pointer goes}
-    struct Plane { const void *from; uint64_t pitch, row, rows, tight; const void **to; };
+    const uint64_t tight = align16(p.sample_bytes() * width);
     PictureSrc dev = p;
-    Plane planes[4];
-    int n = 0;
-    if (is_planar_src(p.kind)) {
-        const uint64_t crow = p.sample_bytes() * (p.alpha_only ? 0 : p.chroma_width(width)), ctight = align16(crow);
-        dev.chroma_pitch = ctight;
-        if (p.alpha_only) {
-            planes[n++] = {p.alpha, pitch, row, height, tight, &dev.alpha};
-        } else {
-            planes[n++] = {p.pixels, pitch, row, height, tight, &dev.pixels};
-            planes[n++] = {p.chroma, p.chroma_pitch, crow, p.chroma_height(height), ctight, &dev.chroma};
-            planes[n++] = {p.cr, p.chroma_pitch, crow, p.chroma_height(height), ctight, &dev.cr};
-            if (p.alpha) planes[n++] = {p.alpha, pitch, row, height, tight, &dev.alpha};
-        }
-    } else {
-        planes[n++] = {p.pixels, pitch, row, height, tight, &dev.pixels};
-        if (p.planes() == 2) planes[n++] = {p.chroma, pitch, row, height / 2, tight, &dev.chroma};
-    }
+    if (p.is_planar()) dev.chroma_pitch = align16(p.sample_bytes() * (p.alpha_only ? 0 : p.chroma_width(width)));
+    PicturePlane<PictureSrc> planes[4];
+    const int n = picture_planes(p, width, height, pitch, planes);
     uint64_t plane_bytes = 0;
     for (int i = 0; i < n; i++) plane_bytes += planes[i].tight * planes[i].rows;
     if (!img.alloc(plane_bytes) || !frame.alloc(align16(cap)) || !used.alloc(32)) { cudaGetLastError(); return HapResult_Internal_Error; }
     uint64_t at = 0;
     for (int i = 0; i < n; i++) {
-        const Plane &q = planes[i];
-        *q.to = img.as<uint8_t>() + at;
-        if (cudaMemcpy2DAsync(img.as<uint8_t>() + at, q.tight, q.from, q.pitch, q.row, q.rows, cudaMemcpyDefault, st) != cudaSuccess) {
+        const PicturePlane<PictureSrc> &q = planes[i];
+        dev.*q.field = img.as<uint8_t>() + at;
+        if (cudaMemcpy2DAsync(img.as<uint8_t>() + at, q.tight, p.*q.field, q.pitch, q.row, q.rows, cudaMemcpyDefault, st) != cudaSuccess) {
             cudaGetLastError();
             return HapResult_Internal_Error;
         }
@@ -1063,6 +1167,32 @@ PictureDst yuv_out_picture(void *luma, void *chroma, unsigned layout, unsigned c
     return {layout == HapB200YUV_P010 ? kDstP010 : kDstNv12, luma, chroma, colorSpace};
 }
 
+// the subsamplings, depths and colour spaces the planar decoders take (BT.601 / BT.709; no BT.2020)
+bool planar_out_args_ok(unsigned subsampling, unsigned bitDepth, unsigned colorSpace)
+{
+    return subsampling <= HapB200Chroma_444 && (bitDepth == 8 || bitDepth == 10 || bitDepth == 12) && colorSpace <= HapB200YUV_BT709_Full;
+}
+
+PictureDst planar_out_picture(void *luma, void *cb, void *cr, void *alpha, unsigned long chromaPitch, unsigned subsampling, unsigned bitDepth,
+                              unsigned colorSpace)
+{
+    PictureDst d{planar_dst(subsampling, bitDepth > 8), luma, cb, colorSpace};
+    d.cr = cr;
+    d.alpha = alpha;
+    d.chroma_pitch = chromaPitch;
+    d.bit_depth = bitDepth;
+    return d;
+}
+
+// Hap Alpha-Only's form of a planar picture: its alpha plane alone (pixels, chroma and cr point at it; nullptr without one)
+PictureDst alpha_only_picture(const PictureDst &d)
+{
+    PictureDst a = d;
+    a.alpha_only = true;
+    a.pixels = a.chroma = a.cr = d.alpha;
+    return a;
+}
+
 // the Hap HDR batch decoders' codec: each frame's signedness comes from its own texture format (frame_formats)
 CodecInfo hap_hdr_batch_codec()
 {
@@ -1137,21 +1267,25 @@ unsigned decode_picture_batch(const CodecInfo &ci, const PictureDst &d, const vo
 }
 
 // One frame in host or device memory -> the picture d.  The frame's codec comes from its headers: Hap HDR frames decode to the
-// RGBA16F and HDR10 sinks only, the other flavours to the others (Bad_Frame otherwise).  Its textures, t[i] bytes each, are
-// decoded by HapDecode into device scratch (a texture that does not fill its room: Bad_Frame; the HDR sinks answer Bad_Frame
-// for one too large for it as well, the others what HapDecode answers); then launch_block_decode writes a tight picture (rows
-// sample_bytes * width apart, the chroma plane's height / 2 rows behind luma's), which is copied to the caller's planes.
-uint32_t decode_picture(const PictureDst &d, const void *inputBuffer, unsigned long inputBufferBytes, unsigned width, unsigned height,
+// RGBA16F and HDR10 sinks only, the other flavours to the others (Bad_Frame otherwise).  A planar picture takes Hap Alpha-Only's
+// form (alpha_only_picture) for a Hap Alpha-Only frame, so before the headers are read its planes need only pass as either
+// form, and after it as the frame's (Bad_Arguments: a Hap Alpha-Only frame without an alpha plane, another without luma, Cb or
+// Cr).  The frame's textures, t[i] bytes each, are decoded by HapDecode into device scratch (a texture that does not fill its
+// room: Bad_Frame; the HDR sinks answer Bad_Frame for one too large for it as well, the others what HapDecode answers); then
+// launch_block_decode writes a tight picture (picture_planes), which is copied to the caller's planes.
+uint32_t decode_picture(const PictureDst &dst, const void *inputBuffer, unsigned long inputBufferBytes, unsigned width, unsigned height,
                         unsigned long pitch)
 {
-    if (!inputBuffer || !picture_geometry_ok(d, width, height, pitch, 0, false)) return HapResult_Bad_Arguments;
+    if (!inputBuffer || !(picture_geometry_ok(dst, width, height, pitch, 0, false) ||
+                          (dst.is_planar() && picture_geometry_ok(alpha_only_picture(dst), width, height, pitch, 0, false))))
+        return HapResult_Bad_Arguments;
     unsigned count = 0, f0 = 0, f1 = 0;
     uint32_t r = HapGetFrameTextureCount(inputBuffer, inputBufferBytes, &count);
     if (r != HapResult_No_Error) return r;
     r = HapGetFrameTextureFormat(inputBuffer, inputBufferBytes, 0, &f0);
     if (r != HapResult_No_Error) return r;
     CodecInfo ci;
-    if (d.hdr()) {
+    if (dst.hdr()) {
         if (count != 1 || !bc6h_codec(f0, ci)) return HapResult_Bad_Frame;
     } else {
         if (count == 2 && (r = HapGetFrameTextureFormat(inputBuffer, inputBufferBytes, 1, &f1)) != HapResult_No_Error) return r;
@@ -1159,13 +1293,18 @@ uint32_t decode_picture(const PictureDst &d, const void *inputBuffer, unsigned l
         while (codec_info(codec, ci) && (ci.textures != count || ci.fmt[0] != f0 || (count == 2 && ci.fmt[1] != f1))) codec++;
         if (!codec_info(codec, ci)) return HapResult_Bad_Frame;
     }
+    const PictureDst d = dst.is_planar() && ci.bc_kind == kBcRgtc1 ? alpha_only_picture(dst) : dst;
+    if (d.is_planar() && !picture_geometry_ok(d, width, height, pitch, 0, false)) return HapResult_Bad_Arguments;
     HAP_ENTER(inputBuffer, d.pixels, d.chroma);
     const uint64_t t[2] = {texture_bytes(width, height, ci, 0), texture_bytes(width, height, ci, 1)};
-    const uint64_t tight = d.sample_bytes() * width, first = tight * height, second = d.planes() == 2 ? tight * (height / 2) : 0;
+    PicturePlane<PictureDst> planes[4];
+    const int n = picture_planes(d, width, height, pitch, planes);
+    uint64_t plane_bytes = 0;
+    for (int i = 0; i < n; i++) plane_bytes += planes[i].tight * planes[i].rows;
     // scratch from the device's stream-ordered pool on the legacy stream (the nested HapDecode calls below write it on
     // that stream, or on a pooled stream they synchronise before returning): no cudaMalloc/cudaFree, no device-wide sync
     DevBuf texb(kLegacyStream), imgb(kLegacyStream);
-    if (!texb.alloc(align16(t[0]) + align16(t[1]) + 16) || !imgb.alloc(first + second)) { cudaGetLastError(); return HapResult_Internal_Error; }
+    if (!texb.alloc(align16(t[0]) + align16(t[1]) + 16) || !imgb.alloc(plane_bytes)) { cudaGetLastError(); return HapResult_Internal_Error; }
     if (cudaStreamSynchronize(kLegacyStream) != cudaSuccess) { cudaGetLastError(); return HapResult_Internal_Error; }   // the allocations are real now
     auto serial = [](HapDecodeWorkFunction fn, void *p, unsigned n, void *) { for (unsigned i = 0; i < n; i++) fn(p, i); };
     for (unsigned i = 0; i < ci.textures && r == HapResult_No_Error; i++) {
@@ -1180,13 +1319,23 @@ uint32_t decode_picture(const PictureDst &d, const void *inputBuffer, unsigned l
     CallStream call(false);  // the scratch buffers are device memory filled on the legacy stream by HapDecode above
     cudaStream_t st = call.st;
     PictureDst img = d;
-    img.pixels = imgb.p;
-    img.chroma = d.planes() == 2 ? imgb.as<uint8_t>() + first : nullptr;
-    r = launch_block_decode(ci, img, texb.as<uint8_t>(), align16(t[0]), 1, 0, width, height, 0, tight, nullptr, nullptr, st);
-    if (r == HapResult_No_Error &&
-        (cudaMemcpy2DAsync(d.pixels, pitch, imgb.p, tight, tight, height, cudaMemcpyDefault, st) != cudaSuccess ||
-         (second && cudaMemcpy2DAsync(d.chroma, pitch, imgb.as<uint8_t>() + first, tight, tight, height / 2, cudaMemcpyDefault, st) != cudaSuccess) ||
-         cudaStreamSynchronize(st) != cudaSuccess)) { cudaGetLastError(); r = HapResult_Internal_Error; }
+    uint64_t at = 0;
+    for (int i = 0; i < n; i++) {
+        img.*planes[i].field = imgb.as<uint8_t>() + at;
+        at += planes[i].tight * planes[i].rows;
+    }
+    if (img.alpha_only) img.pixels = img.chroma = img.cr = img.alpha;
+    if (img.is_planar()) img.chroma_pitch = align16(d.sample_bytes() * (d.alpha_only ? 0 : d.chroma_width(width)));
+    r = launch_block_decode(ci, img, texb.as<uint8_t>(), align16(t[0]), 1, 0, width, height, 0, align16(d.sample_bytes() * width), nullptr,
+                            nullptr, st);
+    for (int i = 0; i < n && r == HapResult_No_Error; i++) {
+        const PicturePlane<PictureDst> &q = planes[i];
+        if (cudaMemcpy2DAsync(d.*q.field, q.pitch, img.*q.field, q.tight, q.row, q.rows, cudaMemcpyDefault, st) != cudaSuccess) {
+            cudaGetLastError();
+            r = HapResult_Internal_Error;
+        }
+    }
+    if (r == HapResult_No_Error && cudaStreamSynchronize(st) != cudaSuccess) { cudaGetLastError(); r = HapResult_Internal_Error; }
     return r;
 }
 
@@ -1904,6 +2053,43 @@ unsigned int HapB200DecodeYUV(const void *inputBuffer, unsigned long inputBuffer
 {
     if (!yuv_out_args_ok(layout, colorSpace)) return HapResult_Bad_Arguments;
     return decode_picture(yuv_out_picture(luma, chroma, layout, colorSpace), inputBuffer, inputBufferBytes, width, height, pitch);
+}
+
+// ---- Hap, Hap Alpha, Hap Q, Hap Q Alpha, Hap Alpha-Only, Hap R -> planar Y'CbCr 4:2:0 / 4:2:2 / 4:4:4 (+ alpha): K8 with a
+// planar sink (planar_sink.cuh); Hap Alpha-Only writes its alpha plane alone --------------------------------------------------
+
+unsigned int HapB200BlockDecodePlanarBatch(const void *blocks, unsigned int frames, unsigned long blocksStride, unsigned int width,
+                                           unsigned int height, unsigned int codec, void *luma, void *cb, void *cr, void *alpha,
+                                           unsigned long frameStride, unsigned long lumaPitch, unsigned long chromaPitch,
+                                           unsigned int subsampling, unsigned int bitDepth, unsigned int colorSpace, void *stream)
+{
+    CodecInfo ci;
+    if (!codec_info(codec, ci) || !planar_out_args_ok(subsampling, bitDepth, colorSpace)) return HapResult_Bad_Arguments;
+    const PictureDst d = planar_out_picture(luma, cb, cr, alpha, chromaPitch, subsampling, bitDepth, colorSpace);
+    return block_decode_picture_batch(ci, ci.bc_kind == kBcRgtc1 ? alpha_only_picture(d) : d, blocks, frames, blocksStride, width, height,
+                                      frameStride, lumaPitch, stream);
+}
+
+unsigned int HapB200DecodePlanarBatch(const void *in, unsigned int frames, unsigned long inStride, const unsigned long long *inBytes,
+                                      unsigned int maxChunks, unsigned int codec, unsigned int width, unsigned int height,
+                                      void *luma, void *cb, void *cr, void *alpha, unsigned long frameStride,
+                                      unsigned long lumaPitch, unsigned long chromaPitch, unsigned int subsampling,
+                                      unsigned int bitDepth, unsigned int colorSpace, unsigned int *results, void *stream)
+{
+    CodecInfo ci;
+    if (!codec_info(codec, ci) || !planar_out_args_ok(subsampling, bitDepth, colorSpace)) return HapResult_Bad_Arguments;
+    const PictureDst d = planar_out_picture(luma, cb, cr, alpha, chromaPitch, subsampling, bitDepth, colorSpace);
+    return decode_picture_batch(ci, ci.bc_kind == kBcRgtc1 ? alpha_only_picture(d) : d, in, frames, inStride, inBytes, maxChunks, width,
+                                height, frameStride, lumaPitch, results, stream);
+}
+
+unsigned int HapB200DecodePlanar(const void *inputBuffer, unsigned long inputBufferBytes, unsigned int width, unsigned int height,
+                                 void *luma, void *cb, void *cr, void *alpha, unsigned long lumaPitch, unsigned long chromaPitch,
+                                 unsigned int subsampling, unsigned int bitDepth, unsigned int colorSpace)
+{
+    if (!planar_out_args_ok(subsampling, bitDepth, colorSpace)) return HapResult_Bad_Arguments;
+    return decode_picture(planar_out_picture(luma, cb, cr, alpha, chromaPitch, subsampling, bitDepth, colorSpace), inputBuffer,
+                          inputBufferBytes, width, height, lumaPitch);
 }
 
 // ---- Hap HDR -> RGBA16F: BC6H (bc6h_decode.cuh) ----

@@ -100,6 +100,12 @@ class HapB200(HapABI):
         L.HapB200DecodeYUVBatch.argtypes = [vp, u, ul, vp, u, u, u, u, vp, vp, ul, ul, u, u, vp, vp]
         L.HapB200BlockDecodeYUVBatch.restype = u
         L.HapB200BlockDecodeYUVBatch.argtypes = [vp, u, ul, u, u, u, vp, vp, ul, ul, u, u, vp]
+        L.HapB200DecodePlanar.restype = u
+        L.HapB200DecodePlanar.argtypes = [vp, ul, u, u, vp, vp, vp, vp, ul, ul, u, u, u]
+        L.HapB200DecodePlanarBatch.restype = u
+        L.HapB200DecodePlanarBatch.argtypes = [vp, u, ul, vp, u, u, u, u, vp, vp, vp, vp, ul, ul, ul, u, u, u, vp, vp]
+        L.HapB200BlockDecodePlanarBatch.restype = u
+        L.HapB200BlockDecodePlanarBatch.argtypes = [vp, u, ul, u, u, u, vp, vp, vp, vp, ul, ul, ul, u, u, u, vp]
         L.HapB200EncodeYUVPQ.restype = u
         L.HapB200EncodeYUVPQ.argtypes = [vp, vp, u, u, ul, u, u, u, u, u, vp, ul, C.POINTER(ul)]
         L.HapB200EncodeYUVPQBatch.restype = u
@@ -374,6 +380,40 @@ class HapB200(HapABI):
                                stream=None):
         return int(self.lib.HapB200BlockDecodeYUVBatch(blocks, frames, blocks_stride, w, h, codec, luma, chroma, frame_stride, pitch, layout,
                                                        color_space, stream))
+
+    # -- Hap (every codec but Hap HDR) -> planar Y'CbCr (+ alpha): subsampling HapB200Chroma_*, bit_depth 8 / 10 / 12 (10 and 12:
+    #    little-endian 16-bit words, sample in the low bits), color_space BT.601 / BT.709 (no BT.2020); pitches as for
+    #    encode_planar; alpha None: no alpha is written; HapA writes alpha alone (luma, cb, cr may be None)
+    def decode_planar(self, frame, w, h, subsampling, bit_depth, color_space, *, with_alpha=True, luma=None, cb=None, cr=None, alpha=None,
+                      luma_pitch=None, chroma_pitch=None, frame_bytes=None):
+        """frame and the planes: buffer objects, (addr, nbytes) or None.  When no plane is given they are allocated here, the
+        alpha plane only when with_alpha.  Returns (result, (luma, cb, cr, alpha or None) bytes) when it allocated the planes and
+        the call succeeded, else (result, None)."""
+        from .abi import _as_ptr
+        lp, cp = self._planar_pitches(w, subsampling, bit_depth, luma_pitch, chroma_pitch)
+        rows = h // 2 if subsampling == HapB200Chroma_420 else h
+        planes = [luma, cb, cr, alpha]
+        own = all(p is None for p in planes)
+        if own:
+            planes = [bytearray(lp * h), bytearray(cp * rows), bytearray(cp * rows), bytearray(lp * h) if with_alpha else None]
+        faddr, fn = _as_ptr(frame)
+        r = int(self.lib.HapB200DecodePlanar(faddr, fn if frame_bytes is None else frame_bytes, w, h,
+                                             *[0 if p is None else _as_ptr(p)[0] for p in planes], lp, cp, subsampling, bit_depth,
+                                             color_space))
+        if not (own and r == 0):
+            return r, None
+        return r, tuple(None if p is None else bytes(p) for p in planes)
+
+    def decode_planar_batch(self, frames_ptr, frames, in_stride, in_bytes, max_chunks, codec, w, h, luma, cb, cr, alpha, frame_stride,
+                            luma_pitch, chroma_pitch, subsampling, bit_depth, color_space, results, stream=None):
+        return int(self.lib.HapB200DecodePlanarBatch(frames_ptr, frames, in_stride, in_bytes, max_chunks, codec, w, h, luma, cb, cr, alpha,
+                                                     frame_stride, luma_pitch, chroma_pitch, subsampling, bit_depth, color_space, results,
+                                                     stream))
+
+    def block_decode_planar_batch(self, blocks, frames, blocks_stride, w, h, codec, luma, cb, cr, alpha, frame_stride, luma_pitch,
+                                  chroma_pitch, subsampling, bit_depth, color_space, stream=None):
+        return int(self.lib.HapB200BlockDecodePlanarBatch(blocks, frames, blocks_stride, w, h, codec, luma, cb, cr, alpha, frame_stride,
+                                                          luma_pitch, chroma_pitch, subsampling, bit_depth, color_space, stream))
 
     # -- HDR10 P010 (BT.2020, PQ) -> Hap HDR (BC6H): color_space HapB200YUV_BT2020_*, unit_nits the cd/m2 of 1.0 (1-10000),
     #    texture_format UF16 or SF16; planes as for encode_yuv with HapB200YUV_P010 (pitch default 2 * width); frames need

@@ -458,6 +458,75 @@ unsigned int HapB200BlockDecodeYUVBatch(const void *blocks, unsigned int frames,
                                         unsigned int height, unsigned int codec, void *luma, void *chroma, unsigned long frameStride,
                                         unsigned long pitch, unsigned int layout, unsigned int colorSpace, void *stream);
 
+/* ---- Hap, Hap Alpha, Hap Q, Hap Q Alpha, Hap Alpha-Only, Hap R -> planar Y'CbCr 4:2:0 / 4:2:2 / 4:4:4 (+ alpha) ------------
+ * The decoders write the planar pictures software encoders and mastering formats take (FFmpeg's yuv420p, yuv422p10le,
+ * yuva444p12le, gray12le and their kin): the inverse of the planar encoders above.  The conversion is fused into the block
+ * decoder, so no RGBA picture is ever written.  The planes are exactly the conversion below applied to the RGBA8 picture that
+ * HapB200DecodeRGBA / HapB200DecodeRGBABatch / HapB200BlockDecodeBatch give for the same input, alpha included.
+ * Arguments, planes, samples and geometry: those of the planar encoders (luma, cb, cr and alpha are AVFrame's data[0..3],
+ * lumaPitch and chromaPitch its linesize[0] and linesize[1]; alpha rows are lumaPitch apart; cw x ch chroma samples; bitDepth
+ * 8: bytes, 10 or 12: little-endian 16-bit words holding the sample in the low bits, the high bits written as zero; width and
+ * height multiples of 4, width*bytes <= lumaPitch <= HAPB200_MAX_ROW_BYTES, cw*bytes <= chromaPitch <= HAPB200_MAX_ROW_BYTES,
+ * at most HAPB200_MAX_BLOCKS blocks).  In a batch, each plane of frame f starts at its pointer + f*frameStride.  The batch
+ * entry points take device pointers; the planes, both pitches, frameStride, blocks and blocksStride are 16-byte aligned.  The
+ * single-frame call takes host or device memory at any alignment and pitch.  Only each row's samples are written: pitch
+ * slack and whatever lies between planes and frames stays as it was.
+ * Codecs: every HapB200Codec.  A non-NULL alpha receives the picture's A (Hap Alpha: DXT5 alpha; Hap Q Alpha: its RGTC1
+ * texture; Hap R: BC7 alpha; Hap: 255, or 0 on DXT1's transparent texels; Hap Q: 255); a NULL alpha writes no alpha.  Hap
+ * Alpha-Only writes its matte v to the alpha plane alone, which it requires: luma, cb and cr are neither written nor checked,
+ * and may be NULL.  A Hap Alpha-Only frame (the batch calls: codec HapB200Codec_HapA) with a NULL alpha is refused with
+ * HapResult_Bad_Arguments; the single-frame call learns the codec from the frame's headers and answers this after reading
+ * them, still before anything touches the GPU.  Colour spaces: BT.601 and BT.709, limited and full range.  BT.2020, unknown
+ * subsamplings, depths, colour spaces or codecs and bad geometry are refused with HapResult_Bad_Arguments before anything
+ * touches the GPU.
+ * Results: HapB200DecodePlanar answers exactly as HapB200DecodeRGBA does (Hap HDR (BC6H) frames: HapResult_Bad_Frame);
+ * HapB200DecodePlanarBatch reports in results[f] exactly what HapB200DecodeRGBABatch reports.  A failed frame's RGBA picture is
+ * all zero bytes, so its planes are the conversion of zeros: Y = yOff, Cb = Cr = cOff, alpha 0.
+ * The conversion, exactly (n = bitDepth), extending that of HapB200DecodeYUV; chroma keeps the default siting the planar
+ * encoders' upsampler assumes:
+ *   1. Chroma sums of total weight 8, Rs, Gs and Bs the weighted sums of R, G and B around chroma sample (i, j), column -1
+ *      clamped to 0:
+ *        4:2:0: HapB200DecodeYUV's, weights 1 2 1 over luma columns 2i-1 .. 2i+1 times 1 1 over rows 2j and 2j+1;
+ *        4:2:2: weights 1 2 1 over columns 2i-1 .. 2i+1 on row j alone, times 2;
+ *        4:4:4: 8*R, 8*G, 8*B of pixel (i, j).
+ *      Then Cb = ((cbR*Rs + cbG*Gs + cbB*Bs + 2^18) >> 19) + cOff, Cr likewise; luma is HapB200DecodeYUV's,
+ *      Y = ((yR*R + yG*G + yB*B + 32768) >> 16) + yOff; each result clamped to 0..2^n-1.  Every intermediate is below 2^31.
+ *   2. Rows: n = 8: the NV12 rows of HAPB200_YUV_OUT_COEFFICIENTS; n = 10: its P010 rows (the samples stored unshifted);
+ *      n = 12: the rows of HAPB200_YUV_12BIT_OUT_COEFFICIENTS below, from the same rule with the 12-bit scales of
+ *      HAPB200_YUV_12BIT_COEFFICIENTS (limited range luma offset 256, luma scale 3504, chroma scale 3584; full range offset 0,
+ *      both scales 4095; chroma offset 2048).  Greys map to exactly neutral chroma, 0 and 255 to the nominal black and white.
+ *   3. Alpha: a = (2*(2^n - 1)*A + 255) / 510, integer division: (2^n - 1)*A / 255 rounded to nearest (no tie occurs),
+ *      so 255 gives 2^n - 1; a = A at n = 8.
+ * Round trips: a flat RGB colour converted to 10- or 12-bit Y'CbCr here and back by the planar encoders' conversion returns
+ * exactly, for all 2^24 colours, in all four colour spaces (at 8 bits it does not, as for NV12).  4:4:4 has no chroma filter,
+ * so any RGBA8 picture decoded to 4:4:4 at 10 or 12 bits with alpha converts back through HapB200EncodePlanar*'s conversion to
+ * the identical RGBA8 picture: yuva444p10le and yuva444p12le are lossless against the RGBA8 decoders.  The planar encoders'
+ * alpha rule inverts step 3 exactly at every depth. */
+/* row colorSpace: {yR, yG, yB, cbR, cbG, cbB, crR, crG, crB, yOff, cOff} */
+#define HAPB200_YUV_12BIT_OUT_COEFFICIENTS                                                                                 \
+    {                                                                                                                      \
+        {269262, 528618, 102662, -155423, -305128, 460551, 460551, -385654, -74897, 256, 2048}, /* BT.601 limited */       \
+        {314677, 617777, 119977, -177583, -348633, 526216, 526216, -440640, -85576, 0, 2048},   /* BT.601 full    */       \
+        {191455, 644068, 65019, -105533, -355018, 460551, 460551, -418321, -42230, 256, 2048},  /* BT.709 limited */       \
+        {223747, 752698, 75986, -120579, -405636, 526215, 526216, -477965, -48251, 0, 2048}     /* BT.709 full    */       \
+    }
+
+/* one Hap frame (host or device pointers, any alignment, any pitches) -> one planar picture */
+unsigned int HapB200DecodePlanar(const void *inputBuffer, unsigned long inputBufferBytes, unsigned int width, unsigned int height,
+                                 void *luma, void *cb, void *cr, void *alpha, unsigned long lumaPitch, unsigned long chromaPitch,
+                                 unsigned int subsampling, unsigned int bitDepth, unsigned int colorSpace);
+/* frames x Hap frame (device, as HapB200DecodeRGBABatch) -> frames x picture (device), each plane at its pointer + f*frameStride */
+unsigned int HapB200DecodePlanarBatch(const void *in, unsigned int frames, unsigned long inStride, const unsigned long long *inBytes,
+                                      unsigned int maxChunks, unsigned int codec, unsigned int width, unsigned int height,
+                                      void *luma, void *cb, void *cr, void *alpha, unsigned long frameStride,
+                                      unsigned long lumaPitch, unsigned long chromaPitch, unsigned int subsampling,
+                                      unsigned int bitDepth, unsigned int colorSpace, unsigned int *results, void *stream);
+/* bare textures (device, as HapB200BlockDecodeBatch; HapM: RGTC1 plane at blocks + HapB200TextureBytes(.., 0)) -> pictures */
+unsigned int HapB200BlockDecodePlanarBatch(const void *blocks, unsigned int frames, unsigned long blocksStride, unsigned int width,
+                                           unsigned int height, unsigned int codec, void *luma, void *cb, void *cr, void *alpha,
+                                           unsigned long frameStride, unsigned long lumaPitch, unsigned long chromaPitch,
+                                           unsigned int subsampling, unsigned int bitDepth, unsigned int colorSpace, void *stream);
+
 /* ---- Hap HDR (BC6H, "HapH") <- HDR10 P010 (BT.2020, SMPTE ST 2084 / PQ) --------------------------------------------------
  * The encoders take the P010 pictures a video decoder writes for HEVC Main10 HDR10 and convert them to linear RGBA16F inside
  * the BC6H encoder, so no RGBA16F picture is ever written.  A P010 picture encodes to exactly the bytes

@@ -94,6 +94,7 @@ struct DeviceState {
     int k5_ctas_per_sm = 1;   // resident CTAs of the fragment compressor per SM (its persistent grid is this x sm_count)
     int fused_ctas_per_sm = 1;   // the same for the fused Hap Q encoder (hapq_fused.cuh)
     int fused_place_ctas_per_sm = 1;   // ... and for its variant that writes the frames itself
+    int ws_place_ctas_per_sm = 1;   // ... and for that variant with its fit and compressor in warp groups of their own
     int units_ctas_per_sm = 1;   // ... and for the Snappy decoder's unit kernel (snappy_execute_units_kernel)
 };
 DeviceState g_dev[kMaxDevices];
@@ -123,6 +124,9 @@ void device_init(int dev)
     ok = ok && cudaFuncSetAttribute(hapq_fused_place_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(EncodeSmem)) == cudaSuccess;
     ok = ok && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&d.fused_place_ctas_per_sm, hapq_fused_place_kernel, kEncThreads,
                                                              sizeof(EncodeSmem)) == cudaSuccess;
+    ok = ok && cudaFuncSetAttribute(hapq_ws_place_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(WsSmem)) == cudaSuccess;
+    ok = ok && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&d.ws_place_ctas_per_sm, hapq_ws_place_kernel, kWsThreads, sizeof(WsSmem)) ==
+                   cudaSuccess;
 #if HAPB200_EX_UNIT_KERNEL
     ok = ok && cudaFuncSetAttribute(snappy_execute_units_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(UnitSmem)) == cudaSuccess;
     ok = ok && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&d.units_ctas_per_sm, snappy_execute_units_kernel, kUxThreads,
@@ -131,6 +135,7 @@ void device_init(int dev)
     if (!ok) { cudaGetLastError(); return; }
     if (d.units_ctas_per_sm < 1) d.units_ctas_per_sm = 1;
     if (d.fused_place_ctas_per_sm < 1) d.fused_place_ctas_per_sm = 1;
+    if (d.ws_place_ctas_per_sm < 1) d.ws_place_ctas_per_sm = 1;
     if (d.k5_ctas_per_sm < 1) d.k5_ctas_per_sm = 1;
     if (d.fused_ctas_per_sm < 1) d.fused_ctas_per_sm = 1;
     d.ready = true;
@@ -367,7 +372,8 @@ struct FusedPictures {
 // frames at out + f*out_stride, lengths in used[f].
 // fused: the textures are not there yet; the fused Hap Q encoder fits them from these pictures, writes them to `base` and
 // compresses them in one kernel, in place of the fragment compressor (G must pass fused_hapq_geometry).  Without the offset
-// table it also writes the streams into the frames (hapq_fused_place_kernel), and the place kernel copies raw fragments only.
+// table it also writes the streams into the frames (hapq_ws_place_kernel, or hapq_fused_place_kernel in -DHAPB200_FUSED_WS=0
+// builds), and the place kernel copies raw fragments only.
 uint32_t launch_encode(const uint8_t *base, const FrameGeom &G, uint32_t frames, uint8_t *out, uint64_t out_stride,
                        unsigned long long *used, cudaStream_t st, const FusedPictures *fused = nullptr)
 {
@@ -396,10 +402,17 @@ uint32_t launch_encode(const uint8_t *base, const FrameGeom &G, uint32_t frames,
         }
         uint32_t *sy = sync.as<uint32_t>();
         const FusedPlaceArgs P{out, out_stride, sy, sy + 2, sy + 2 + nfrag};
-        const uint64_t resident = (uint64_t)sm_count() * (uint64_t)g_dev[t_device].fused_place_ctas_per_sm;
-        HAP_KLAUNCH(kStBcEncode, hapq_fused_place_kernel, dim3((unsigned)(nfrag < resident ? nfrag : resident)), dim3(kEncThreads),
-                    sizeof(EncodeSmem), st, fused->rgba, fused->g, const_cast<uint8_t *>(base), G, (uint32_t)nfrag, scratch.as<uint8_t>(),
-                    fsize.as<uint32_t>(), entries, P);
+        if (HAPB200_FUSED_WS) {
+            const uint64_t resident = (uint64_t)sm_count() * (uint64_t)g_dev[t_device].ws_place_ctas_per_sm;
+            HAP_KLAUNCH(kStBcEncode, hapq_ws_place_kernel, dim3((unsigned)(nfrag < resident ? nfrag : resident)), dim3(kWsThreads),
+                        sizeof(WsSmem), st, fused->rgba, fused->g, const_cast<uint8_t *>(base), G, (uint32_t)nfrag, scratch.as<uint8_t>(),
+                        fsize.as<uint32_t>(), entries, P);
+        } else {
+            const uint64_t resident = (uint64_t)sm_count() * (uint64_t)g_dev[t_device].fused_place_ctas_per_sm;
+            HAP_KLAUNCH(kStBcEncode, hapq_fused_place_kernel, dim3((unsigned)(nfrag < resident ? nfrag : resident)), dim3(kEncThreads),
+                        sizeof(EncodeSmem), st, fused->rgba, fused->g, const_cast<uint8_t *>(base), G, (uint32_t)nfrag, scratch.as<uint8_t>(),
+                        fsize.as<uint32_t>(), entries, P);
+        }
         HAP_KLAUNCH(kStPlan, hap_plan_placed_frames_kernel, dim3(frames), dim3(kPlanThreads), 0, st, G, base, fsize.as<uint32_t>(),
                     fdst.as<uint32_t>(), fidx.as<uint32_t>(), plan_flags, out, out_stride, used,
                     PlanPlaced{scratch.as<uint8_t>(), entries, work.as<uint32_t>(), sy + 1});
@@ -1524,6 +1537,22 @@ int HapB200StageTimes(double *ms, unsigned long long *launches, int n)
     cudaGetLastError();
     return kStCount;
 }
+
+#if HAPB200_ENC_PHASE_CLOCKS
+// Measurement builds only (-DHAPB200_ENC_PHASE_CLOCKS=1): the fused Hap Q encoders' clocks per phase summed over every CTA
+// of the current device since the last call, then the fragments compressed (snappy_encode.cuh, kEp*).  Synchronises the
+// device and resets the sums.  Returns the number of slots.
+int HapB200EncodePhaseClocks(unsigned long long *out, int n)
+{
+    cudaDeviceSynchronize();
+    unsigned long long v[kEpSlots] = {};
+    if (cudaMemcpyFromSymbol(v, g_enc_phase_clocks, sizeof v) != cudaSuccess) { cudaGetLastError(); return -1; }
+    const unsigned long long zero[kEpSlots] = {};
+    cudaMemcpyToSymbol(g_enc_phase_clocks, zero, sizeof zero);
+    for (int i = 0; i < n && i < kEpSlots; i++) out[i] = v[i];
+    return kEpSlots;
+}
+#endif
 
 #if HAPB200_EX_PHASE_CLOCKS
 // Measurement builds only (-DHAPB200_EX_PHASE_CLOCKS=1): the unit path's clocks per phase summed over every CTA of the

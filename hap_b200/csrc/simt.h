@@ -66,6 +66,13 @@ __device__ __forceinline__ uint32_t hap_ld_acquire(const uint32_t *p)
 }
 __device__ __forceinline__ void hap_st_release(uint32_t *p, uint32_t v) { asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
 __device__ __forceinline__ void hap_nanosleep(uint32_t ns) { asm volatile("nanosleep.u32 %0;" ::"r"(ns)); }
+
+// ---- named barriers (warp groups of one CTA) ------------------------------------------------------------------------
+// Barrier `id` (1..15; 0 is __syncthreads) completes once `n` threads (a multiple of 32, whole warps) have arrived.  sync
+// waits for that; arrive only counts this warp and goes on.  Shared-memory writes before an arrive are seen by the threads
+// behind the sync that completes the same barrier phase (the producer / consumer hand-off).
+__device__ __forceinline__ void hap_bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+__device__ __forceinline__ void hap_bar_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 #endif
 
 #define HAP_FULL_MASK 0xffffffffu

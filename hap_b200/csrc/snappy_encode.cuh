@@ -63,6 +63,62 @@ struct EncodeSmem {
 // may use (233,472 - 2 x 1,024) / 2 = 115,712 bytes.
 static_assert(sizeof(EncodeSmem) <= 115712, "two encode CTAs fit the shared memory of one SM");
 
+// -DHAPB200_ENC_PHASE_CLOCKS=1 (measurement builds only, tools/measure_enc_phases.py): thread 0 of the compressor (and,
+// in hapq_ws_place_kernel, thread 0 of the fit group, thread kEncThreads) adds up clock64() per phase of the fused Hap Q
+// encoders in shared memory, and thread 0 folds the sums into g_enc_phase_clocks when the CTA ends.  Phases end at barriers
+// where there is one, so a phase's clocks are those of its warp group, not of one thread alone.
+#ifndef HAPB200_ENC_PHASE_CLOCKS
+#define HAPB200_ENC_PHASE_CLOCKS 0
+#endif
+enum : int {
+    kEpFit = 0,          // the fit
+    kEpFitWait,          // the barrier behind the fit (hapq_ws_place_kernel: the compressor waits for a fitted image)
+    kEpHash, kEpCandidates, kEpPropagate, kEpRunScan, kEpSizeScan, kEpWrite,   // compress_fragment's steps 1 .. 5
+    kEpLookBack,         // the look-back of the fragment whose stream waits in shared memory, and the barrier behind it
+    kEpStore,            // its stream to the frame
+    kEpOther,            // table clear, strip load, ticket, size publication
+    kEpGroupFit,         // hapq_ws_place_kernel's fit group: fitting
+    kEpGroupEmptyWait,   // ... waiting for the compressor to release an image
+    kEpGroupTicket,      // ... handing out the ticket inside the group
+    kEpCount
+};
+enum : int { kEpFragments = kEpCount, kEpSlots };   // fragments compressed, kept behind the phase clocks
+#if HAPB200_ENC_PHASE_CLOCKS && !defined(HAPB200_EMU)
+__device__ unsigned long long g_enc_phase_clocks[kEpSlots];
+__shared__ unsigned long long s_enc_phase[kEpSlots + 2];   // [kEpSlots + w]: clock of warp group w's last mark
+#define HAP_EPHASE_BEGIN()                                                                \
+    do {                                                                                  \
+        if (threadIdx.x == 0)                                                             \
+            for (int q_ = 0; q_ < kEpSlots; q_++) s_enc_phase[q_] = 0;                    \
+        __syncthreads();                                                                  \
+        if ((threadIdx.x & (kEncThreads - 1)) == 0) s_enc_phase[kEpSlots + threadIdx.x / kEncThreads] = clock64(); \
+    } while (0)
+#define HAP_EPHASE_MARK(ph)                                                               \
+    do {                                                                                  \
+        if ((threadIdx.x & (kEncThreads - 1)) == 0) {                                     \
+            const unsigned long long c_ = clock64();                                      \
+            unsigned long long &l_ = s_enc_phase[kEpSlots + threadIdx.x / kEncThreads];   \
+            s_enc_phase[ph] += c_ - l_;                                                   \
+            l_ = c_;                                                                      \
+        }                                                                                 \
+    } while (0)
+#define HAP_EPHASE_COUNT(slot)                                                            \
+    do {                                                                                  \
+        if (threadIdx.x == 0) s_enc_phase[slot]++;                                        \
+    } while (0)
+#define HAP_EPHASE_END()                                                                  \
+    do {                                                                                  \
+        __syncthreads();                                                                  \
+        if (threadIdx.x == 0)                                                             \
+            for (int q_ = 0; q_ < kEpSlots; q_++) atomicAdd(&g_enc_phase_clocks[q_], s_enc_phase[q_]); \
+    } while (0)
+#else
+#define HAP_EPHASE_BEGIN() do {} while (0)
+#define HAP_EPHASE_MARK(ph) do {} while (0)
+#define HAP_EPHASE_COUNT(slot) do {} while (0)
+#define HAP_EPHASE_END() do {} while (0)
+#endif
+
 __device__ __forceinline__ uint32_t enc_hash(uint2 u) { return ((u.x * 0x9E3779B1u) ^ (u.y * 0x85EBCA6Bu)) >> (32 - kEncHashBits); }
 __device__ __forceinline__ bool same_unit(uint2 a, uint2 b) { return a.x == b.x && a.y == b.y; }
 
@@ -73,9 +129,20 @@ __device__ __forceinline__ void store_strip16(uint16_t *arr, uint32_t base, cons
     *reinterpret_cast<uint4 *>(arr + base) = make_uint4(v[0] | (v[1] << 16), v[2] | (v[3] << 16), v[4] | (v[5] << 16), v[6] | (v[7] << 16));
 }
 
+// The barrier the compressor's kEncThreads threads meet at: the whole CTA (K5, the fused kernels), or a named barrier of
+// the compressor's warp group when the CTA has other warps too (hapq_ws_place_kernel).
+struct CtaBarrier {
+    __device__ static __forceinline__ void sync() { __syncthreads(); }
+};
+template <int ID>
+struct GroupBarrier {
+    __device__ static __forceinline__ void sync() { hap_bar_sync(ID, kEncThreads); }
+};
+
 // Inclusive max / sum over the block of one value per thread; returns the exclusive prefix for this thread and
 // the block total.  Two barriers.  The warp totals are scanned by every warp with shuffles (lane w holds the
 // total of warp w; lanes past the last warp hold the identity, 0 for both) instead of a loop over shared memory.
+template <class Bar = CtaBarrier>
 __device__ __forceinline__ uint32_t enc_block_excl(uint32_t v, bool is_max, uint32_t *total, uint32_t *warp_tot)
 {
     static_assert(kEncWarps <= 32, "one warp total per lane");
@@ -89,7 +156,7 @@ __device__ __forceinline__ uint32_t enc_block_excl(uint32_t v, bool is_max, uint
     uint32_t prev = __shfl_up_sync(HAP_FULL_MASK, incl, 1);
     if (lane == 0) prev = 0;
     if (lane == 31) warp_tot[warp] = incl;
-    __syncthreads();
+    Bar::sync();
     uint32_t wi = lane < kEncWarps ? warp_tot[lane] : 0u;
 #pragma unroll
     for (int d = 1; d < 32; d <<= 1) {
@@ -99,18 +166,20 @@ __device__ __forceinline__ uint32_t enc_block_excl(uint32_t v, bool is_max, uint
     const uint32_t tot = __shfl_sync(HAP_FULL_MASK, wi, 31);
     uint32_t base = __shfl_sync(HAP_FULL_MASK, wi, warp > 0 ? warp - 1 : 0);
     if (warp == 0) base = 0;
-    __syncthreads();
+    Bar::sync();
     *total = tot;
     return is_max ? (base > prev ? base : prev) : base + prev;
 }
 
-// One fragment: U units (8 bytes each; U <= kFragUnits) already in S.data AND in the caller's registers d[8] (units
-// 8t..8t+7) -> element stream written to S.out as bytes; returns its size (all threads).
+// One fragment: U units (8 bytes each; U <= kFragUnits) already in the shared-memory image `data` (S.data, or a second
+// image of the same size) AND in the caller's registers d[8] (units 8t..8t+7) -> element stream written to `out` (S.out,
+// or a second buffer of the same size) as bytes; returns its size (all threads).
 // period_units = DXT block size in units (1 or 2).
 // FULL = the fragment has all kFragUnits units (31 of 32 fragments of a 1 MiB chunk): every per-unit bounds test
-// folds away at compile time.
-template <bool FULL>
-__device__ __forceinline__ uint32_t compress_fragment(EncodeSmem &S, const uint2 d[kUnitStrip], uint32_t Udyn, uint32_t period_units)
+// folds away at compile time.  Bar: the barrier of the kEncThreads threads that run it.
+template <bool FULL, class Bar = CtaBarrier>
+__device__ __forceinline__ uint32_t compress_fragment(EncodeSmem &S, const uint2 *data, uint32_t *out_words, const uint2 d[kUnitStrip],
+                                                      uint32_t Udyn, uint32_t period_units)
 {
     const uint32_t t = threadIdx.x;
     const uint32_t U = FULL ? (uint32_t)kFragUnits : Udyn;
@@ -134,7 +203,8 @@ __device__ __forceinline__ uint32_t compress_fragment(EncodeSmem &S, const uint2
             if ((uint32_t)k < nv && !dup) atomicMin(&S.u.table[hsh[k]], i0 + k);
         }
     }
-    __syncthreads();
+    Bar::sync();
+    HAP_EPHASE_MARK(kEpHash);
 
     // 2. candidate distance per unit: first earlier occurrence, or one block back when the whole block repeats
     uint32_t dd[kUnitStrip];
@@ -143,25 +213,26 @@ __device__ __forceinline__ uint32_t compress_fragment(EncodeSmem &S, const uint2
         dd[k] = 0;
         if ((uint32_t)k < nv) {
             const uint32_t c = S.u.table[hsh[k]];
-            if (c < i0 + k && same_unit(S.data[c], d[k])) dd[k] = i0 + k - c;
+            if (c < i0 + k && same_unit(data[c], d[k])) dd[k] = i0 + k - c;
         }
     }
     if (period_units == 2) {
         // DXT5-sized blocks: units (2b, 2b+1); the block repeats when both of its units exist and equal the block before
-        const uint2 p0 = i0 >= 2 ? S.data[i0 - 2] : make_uint2(0, 0), p1 = i0 >= 2 ? S.data[i0 - 1] : make_uint2(0, 0);
+        const uint2 p0 = i0 >= 2 ? data[i0 - 2] : make_uint2(0, 0), p1 = i0 >= 2 ? data[i0 - 1] : make_uint2(0, 0);
         if (i0 >= 2 && nv >= 2 && same_unit(p0, d[0]) && same_unit(p1, d[1])) { dd[0] = 2; dd[1] = 2; }
 #pragma unroll
         for (int k = 2; k < kUnitStrip; k += 2)
             if ((uint32_t)k + 2 <= nv && same_unit(d[k - 2], d[k]) && same_unit(d[k - 1], d[k + 1])) { dd[k] = 2; dd[k + 1] = 2; }
     } else {
-        const uint2 p = i0 >= 1 ? S.data[i0 - 1] : make_uint2(0, 0);
+        const uint2 p = i0 >= 1 ? data[i0 - 1] : make_uint2(0, 0);
         if (i0 >= 1 && nv >= 1 && same_unit(p, d[0])) dd[0] = 1;
 #pragma unroll
         for (int k = 1; k < kUnitStrip; k++)
             if ((uint32_t)k < nv && same_unit(d[k - 1], d[k])) dd[k] = 1;
     }
     store_strip16(S.da, i0, dd);
-    __syncthreads();
+    Bar::sync();
+    HAP_EPHASE_MARK(kEpCandidates);
 
     // 2b. propagation (one round): a unit that is not yet part of a run adopts its left (else right) neighbour's
     //     distance when its own data also matches there.  First occurrences of neighbouring units often point at
@@ -180,8 +251,8 @@ __device__ __forceinline__ uint32_t compress_fragment(EncodeSmem &S, const uint2
             if ((uint32_t)k < nv && !(cd != 0 && (cd == l || cd == r))) {
                 // one look-up decides: the left neighbour's distance if there is one, else the right one's
                 const uint32_t cand = l != 0 ? l : r;
-                if (cand != 0 && i >= cand && same_unit(S.data[i - cand], d[k])) dd[k] = cand;
-                else if (l != 0 && r != 0 && r != l && i >= r && same_unit(S.data[i - r], d[k])) dd[k] = r;
+                if (cand != 0 && i >= cand && same_unit(data[i - cand], d[k])) dd[k] = cand;
+                else if (l != 0 && r != 0 && r != l && i >= r && same_unit(data[i - r], d[k])) dd[k] = r;
             }
             l = cd;
         }
@@ -190,7 +261,8 @@ __device__ __forceinline__ uint32_t compress_fragment(EncodeSmem &S, const uint2
     // below and by the re-dealt output step); S.da is free once every thread has read its neighbours there, and takes
     // the run ends.  (A single matching unit is kept: an 8-byte copy costs 3 bytes.)
     store_strip16(S.u.h.a, i0, dd);
-    __syncthreads();
+    Bar::sync();
+    HAP_EPHASE_MARK(kEpPropagate);
     const uint16_t *fin = S.u.h.a;
     uint16_t *ends = S.da;
 
@@ -207,7 +279,7 @@ __device__ __forceinline__ uint32_t compress_fragment(EncodeSmem &S, const uint2
             loc[k] = last;
         }
         uint32_t unused;
-        const uint32_t carry = enc_block_excl(last, true, &unused, S.warp_tot);
+        const uint32_t carry = enc_block_excl<Bar>(last, true, &unused, S.warp_tot);
 #pragma unroll
         for (int k = 0; k < kUnitStrip; k++) rs[k] = (loc[k] ? loc[k] : carry) - 1;
         const uint32_t rb = i0 + kUnitStrip < U ? fin[i0 + kUnitStrip] : 0xFFFFFFFFu;
@@ -217,7 +289,8 @@ __device__ __forceinline__ uint32_t compress_fragment(EncodeSmem &S, const uint2
             if ((uint32_t)k < nv && (i0 + k + 1 == U || nx != dd[k])) ends[rs[k]] = (uint16_t)(i0 + k);
         }
     }
-    __syncthreads();
+    Bar::sync();
+    HAP_EPHASE_MARK(kEpRunScan);
 
     // 4. bytes each unit contributes and their exclusive prefix sum
     uint32_t pos[kUnitStrip];
@@ -239,7 +312,7 @@ __device__ __forceinline__ uint32_t compress_fragment(EncodeSmem &S, const uint2
             run += c;
         }
         uint32_t tot;
-        const uint32_t base = enc_block_excl(run, false, &tot, S.warp_tot);
+        const uint32_t base = enc_block_excl<Bar>(run, false, &tot, S.warp_tot);
 #pragma unroll
         for (int k = 0; k < kUnitStrip; k++) pos[k] += base;
         if (t == 0) S.total = tot;
@@ -253,8 +326,9 @@ __device__ __forceinline__ uint32_t compress_fragment(EncodeSmem &S, const uint2
     //    written bytewise.
     store_strip16(S.u.h.c, i0, pos);
     store_strip16(S.u.h.b, i0, rs);
-    __syncthreads();
-    uint8_t *out = reinterpret_cast<uint8_t *>(S.out);
+    Bar::sync();
+    HAP_EPHASE_MARK(kEpSizeScan);
+    uint8_t *out = reinterpret_cast<uint8_t *>(out_words);
 #pragma unroll 1
     for (int j = 0; j < kUnitStrip; j++) {
         const uint32_t i = t + (uint32_t)j * kEncThreads;
@@ -262,7 +336,7 @@ __device__ __forceinline__ uint32_t compress_fragment(EncodeSmem &S, const uint2
         const uint32_t dist = S.u.h.a[i], rs_i = S.u.h.b[i];
         uint32_t p = S.u.h.c[i];
         if (dist == 0) {
-            const uint2 w = S.data[i];
+            const uint2 w = data[i];
             const uint32_t e = ends[rs_i];   // last unit of this literal run
             if (i == rs_i) {
                 const uint32_t len = 8u * (e - i + 1);
@@ -288,7 +362,7 @@ __device__ __forceinline__ uint32_t compress_fragment(EncodeSmem &S, const uint2
                     for (uint32_t q = 0; q < 4u - sh; q++) out[p + q] = (uint8_t)(w.x >> (8 * q));   // the run's first bytes
                 *reinterpret_cast<uint32_t *>(out + a1) = __funnelshift_r(w.x, w.y, 8 * (4u - sh));
                 if (i < e) {
-                    *reinterpret_cast<uint32_t *>(out + a1 + 4) = __funnelshift_r(w.y, S.data[i + 1].x, 8 * (4u - sh));
+                    *reinterpret_cast<uint32_t *>(out + a1 + 4) = __funnelshift_r(w.y, data[i + 1].x, 8 * (4u - sh));
                 } else {
                     for (uint32_t q = 0; q < sh; q++) out[a1 + 4 + q] = (uint8_t)(w.y >> (8 * (4u - sh + q)));   // the run's last bytes
                 }
@@ -303,7 +377,8 @@ __device__ __forceinline__ uint32_t compress_fragment(EncodeSmem &S, const uint2
             out[p + 2] = (uint8_t)(off >> 8);
         }
     }
-    __syncthreads();
+    Bar::sync();
+    HAP_EPHASE_MARK(kEpWrite);
     return S.total;
 }
 
@@ -453,8 +528,8 @@ __global__ void __launch_bounds__(kEncThreads, 2) snappy_encode_fragments_kernel
         init_fragment_tables(S);
         __syncthreads();
         const uint32_t period_units = (cur.second ? G.s[1].period_words : G.s[0].period_words) >> 1;   // 8-byte blocks: 1, 16-byte blocks: 2
-        const uint32_t total = U == (uint32_t)kFragUnits ? compress_fragment<true>(S, d, U, period_units)
-                                                         : compress_fragment<false>(S, d, U, period_units);
+        const uint32_t total = U == (uint32_t)kFragUnits ? compress_fragment<true>(S, S.data, S.out, d, U, period_units)
+                                                         : compress_fragment<false>(S, S.data, S.out, d, U, period_units);
         store_fragment(S, total, gfrag, scratch, frag_size, frag_entries);
     }
 }

@@ -1,5 +1,5 @@
 // hap_b200/csrc/bc_encode.cuh -- K1-K4 kernels: RGBA8 (or NV12 / P010, or planar Y'CbCr) frames -> DXT1 / DXT5 /
-// scaled-YCoCg-DXT5 / RGTC1 blocks.
+// scaled-YCoCg-DXT5 / RGTC1 / BC7 blocks, and the Y'CbCr -> RGBA8 pass that BC7 takes from Y'CbCr pictures.
 //
 // One thread per 4x4 block (see bc_block.cuh for why).  Memory shape: thread t of a warp owns block
 // column bx0+t, so for each of the four pixel rows the warp reads 32 x 16 B = 512 contiguous bytes
@@ -154,6 +154,42 @@ __global__ void __launch_bounds__(kBcThreads, bc_encode_min_ctas(KIND, REFINE)) 
     constexpr bool kAlpha = KIND == kBcDxt5 || KIND == kBcYCoCgPlusAlpha || KIND == kBcRgtc1;
     load_block_planar<SRC, KIND != kBcRgtc1, kAlpha>(luma + f, G.row_bytes, bx, by, G.blocks_x, G.blocks_y, p, px);
     bc_encode_store<KIND, REFINE>(px, G, out + (uint64_t)blockIdx.y * G.out_stride, bi);
+}
+
+// The first of BC7's two passes from a Y'CbCr picture (Hap R from NV12 / P010 or planar pictures): the picture -> a tight
+// RGBA8 picture, which bc_encode_kernel<kBcBc7> then encodes unchanged.  The DXT kinds fuse the conversion into their fit;
+// BC7 does not, because each source would instantiate the whole BC7 search again (minutes of build and more spills each),
+// and the RGBA8 round trip costs three orders of magnitude less than the search (DESIGN.md section 4).
+// grid = (bc_ctas, frames), one thread per 4x4 block.  The block encoders' own loaders convert (load_block_yuv for
+// kSrcNv12 / kSrcP010, load_block_planar with alpha for kSrcPlanar*), so the picture is exactly the one the DXT encoders fit
+// from.  G: the source (luma rows row_bytes apart, every plane frame_bytes apart per frame); out_stride is the RGBA8 frame
+// stride, its rows 16*blocks_x bytes apart.  Y: the NV12 / P010 chroma plane and matrix; P: the planar ones (alpha nullptr:
+// A = 255).  Each pixel row of the block is one 16-byte store.
+template <int SRC>
+__global__ void __launch_bounds__(kBcThreads) bc_source_to_rgba8_kernel(const uint8_t *__restrict__ luma, BcGeom G, uint8_t *__restrict__ rgba,
+                                                                       YuvSrc Y, PlanarSrc P)
+{
+    const uint32_t nblocks = G.blocks_x * G.blocks_y;
+    const uint32_t bi = blockIdx.x * kBcThreads + threadIdx.x;
+    if (bi >= nblocks) return;
+    uint32_t bx, by;
+    block_xy(bi, G.blocks_x, G.inv_blocks_x, bx, by);
+    const uint64_t f = (uint64_t)blockIdx.y * G.frame_bytes;
+    uint32_t px[16];
+    if constexpr (SRC == kSrcNv12 || SRC == kSrcP010) {
+        load_block_yuv<SRC>(luma + f, Y.chroma + f, G.row_bytes, bx, by, G.blocks_x, G.blocks_y, Y, px);
+    } else {
+        PlanarSrc p = P;
+        p.m.chroma += f;
+        p.cr += f;
+        if (p.alpha) p.alpha += f;
+        load_block_planar<SRC, true, true>(luma + f, G.row_bytes, bx, by, G.blocks_x, G.blocks_y, p, px);
+    }
+    const uint64_t row = 16ull * G.blocks_x;
+    uint8_t *o = rgba + (uint64_t)blockIdx.y * G.out_stride + 4 * by * row + 16ull * bx;
+#pragma unroll
+    for (int r = 0; r < 4; r++)
+        *reinterpret_cast<uint4 *>(o + r * row) = make_uint4(px[4 * r + 0], px[4 * r + 1], px[4 * r + 2], px[4 * r + 3]);
 }
 
 }  // namespace hapb200

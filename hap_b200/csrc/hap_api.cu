@@ -599,6 +599,54 @@ void launch_bc6h_slices(uint32_t frames, cudaStream_t st, const uint8_t *rgba, c
     }
 }
 
+// The RGBA8 scratch of BC7 from a Y'CbCr picture holds at most this many bytes, or one frame when a frame is larger
+constexpr uint64_t kBc7ScratchBytes = 256ull << 20;
+
+// The BC7 kind of launch_block_encode from NV12 / P010 or planar pictures (g: their geometry, out_stride the blocks' frame
+// stride), in two passes per slice of frames: bc_source_to_rgba8_kernel converts the slice into a tight RGBA8 picture in
+// scratch, then the RGBA8 BC7 kernel encodes it, so no BC7 search is instantiated per source (bc_encode.cuh).  Whole frames
+// per slice, as many as kBc7ScratchBytes holds (at least one); stream order lets each slice reuse the scratch.
+uint32_t launch_bc7_from_yuv(uint32_t frames, cudaStream_t st, const uint8_t *luma, const BcGeom &g, uint8_t *blocks, int src,
+                             const YuvSrc &yuv, const PlanarSrc &planar)
+{
+    const uint64_t row = 16ull * g.blocks_x, frame_rgba = row * 4 * g.blocks_y;   // (the entry points: 4 * width < 2^32)
+    uint64_t slice = kBc7ScratchBytes / frame_rgba;
+    slice = slice < 1 ? 1 : slice > kBcFramesPerLaunch ? kBcFramesPerLaunch : slice;
+    if (slice > frames) slice = frames;
+    DevBuf rgba(st);
+    if (!rgba.alloc(slice * frame_rgba)) { cudaGetLastError(); return HapResult_Internal_Error; }
+    BcGeom cg = g;   // the source read, the RGBA8 picture written
+    cg.out_stride = frame_rgba;
+    const BcGeom rg = bc_encode_geom(4 * g.blocks_x, 4 * g.blocks_y, (uint32_t)row, frame_rgba, g.out_stride, 0);
+    for (uint32_t f0 = 0; f0 < frames; f0 += (uint32_t)slice) {
+        const uint32_t n = frames - f0 < slice ? frames - f0 : (uint32_t)slice;
+        const dim3 grid(bc_ctas(g.blocks_x, g.blocks_y), n);
+        const uint8_t *s = luma + f0 * g.frame_bytes;
+        YuvSrc y = yuv;
+        PlanarSrc p = planar;
+        if (y.chroma) y.chroma += f0 * g.frame_bytes;
+        if (is_planar_src(src)) {
+            p.m.chroma += f0 * g.frame_bytes;
+            p.cr += f0 * g.frame_bytes;
+            if (p.alpha) p.alpha += f0 * g.frame_bytes;
+        }
+        uint8_t *o = rgba.as<uint8_t>();
+        switch (src) {
+        case kSrcNv12: HAP_KLAUNCH(kStBcEncode, bc_source_to_rgba8_kernel<kSrcNv12>, grid, dim3(kBcThreads), 0, st, s, cg, o, y, p); break;
+        case kSrcP010: HAP_KLAUNCH(kStBcEncode, bc_source_to_rgba8_kernel<kSrcP010>, grid, dim3(kBcThreads), 0, st, s, cg, o, y, p); break;
+        case kSrcPlanar420x8: HAP_KLAUNCH(kStBcEncode, bc_source_to_rgba8_kernel<kSrcPlanar420x8>, grid, dim3(kBcThreads), 0, st, s, cg, o, y, p); break;
+        case kSrcPlanar420x16: HAP_KLAUNCH(kStBcEncode, bc_source_to_rgba8_kernel<kSrcPlanar420x16>, grid, dim3(kBcThreads), 0, st, s, cg, o, y, p); break;
+        case kSrcPlanar422x8: HAP_KLAUNCH(kStBcEncode, bc_source_to_rgba8_kernel<kSrcPlanar422x8>, grid, dim3(kBcThreads), 0, st, s, cg, o, y, p); break;
+        case kSrcPlanar422x16: HAP_KLAUNCH(kStBcEncode, bc_source_to_rgba8_kernel<kSrcPlanar422x16>, grid, dim3(kBcThreads), 0, st, s, cg, o, y, p); break;
+        case kSrcPlanar444x8: HAP_KLAUNCH(kStBcEncode, bc_source_to_rgba8_kernel<kSrcPlanar444x8>, grid, dim3(kBcThreads), 0, st, s, cg, o, y, p); break;
+        case kSrcPlanar444x16: HAP_KLAUNCH(kStBcEncode, bc_source_to_rgba8_kernel<kSrcPlanar444x16>, grid, dim3(kBcThreads), 0, st, s, cg, o, y, p); break;
+        default: return HapResult_Bad_Arguments;
+        }
+        launch_bc_encode<kBcBc7>(n, st, o, rg, blocks + f0 * g.out_stride, false, kSrcRgba8, YuvSrc(), PlanarSrc());
+    }
+    return cudaGetLastError() == cudaSuccess ? HapResult_No_Error : HapResult_Internal_Error;
+}
+
 // The pictures p (frame f's planes frame_stride apart, luma / RGBA rows row_bytes apart) -> blocks of ci, frame f's at
 // blocks + f*blocks_stride, its second texture (Hap Q Alpha) second_offset behind them.  BC6H signedness: ci.fmt[0].
 uint32_t launch_block_encode(const CodecInfo &ci, const PictureSrc &p, uint32_t frames, uint64_t frame_stride, uint32_t width,
@@ -611,6 +659,8 @@ uint32_t launch_block_encode(const CodecInfo &ci, const PictureSrc &p, uint32_t 
     const YuvSrc yuv = p.yuv();
     const PlanarSrc planar = p.planar();
     const bool refine = g_chroma_refine.load() != 0;
+    if (ci.bc_kind == kBcBc7 && (src == kSrcNv12 || src == kSrcP010 || is_planar_src(src)))
+        return launch_bc7_from_yuv(frames, st, rgba, g, blocks, src, yuv, planar);
     if (src != kSrcRgba8 && ci.bc_kind == kBcBc7) return HapResult_Bad_Arguments;
     if ((src == kSrcNv12 || src == kSrcP010) && ci.bc_kind == kBcRgtc1) return HapResult_Bad_Arguments;
     switch (ci.bc_kind) {
@@ -1126,10 +1176,13 @@ CodecInfo bc7_codec()
     return ci;
 }
 
+// the layouts and colour spaces the YUV encoders take (BC7 from Y'CbCr too)
+bool yuv_format_ok(unsigned layout, unsigned colorSpace) { return layout <= HapB200YUV_P010 && colorSpace <= HapB200YUV_BT709_Full; }
+
 // the codecs the YUV encoders take (every one with a block compressor that encodes colour) and the layouts and colour spaces
 bool yuv_args_ok(unsigned layout, unsigned colorSpace, unsigned codec, CodecInfo &ci)
 {
-    return layout <= HapB200YUV_P010 && colorSpace <= HapB200YUV_BT709_Full && codec_info(codec, ci) && codec_encodes(ci) && ci.bc_kind != kBcRgtc1;
+    return yuv_format_ok(layout, colorSpace) && codec_info(codec, ci) && codec_encodes(ci) && ci.bc_kind != kBcRgtc1;
 }
 
 PictureSrc yuv_picture(const void *luma, const void *chroma, unsigned layout, unsigned colorSpace)
@@ -1137,13 +1190,21 @@ PictureSrc yuv_picture(const void *luma, const void *chroma, unsigned layout, un
     return {layout == HapB200YUV_P010 ? kSrcP010 : kSrcNv12, luma, chroma, colorSpace};
 }
 
-// the codecs (every one with a block compressor; HapA only with an alpha plane), subsamplings, depths and colour spaces the
-// planar encoders take
+// the subsamplings, depths and colour spaces the planar encoders take (BC7 from Y'CbCr too)
+bool planar_format_ok(unsigned subsampling, unsigned bitDepth, unsigned colorSpace)
+{
+    return subsampling <= HapB200Chroma_444 && (bitDepth == 8 || bitDepth == 10 || bitDepth == 12) && colorSpace <= HapB200YUV_BT709_Full;
+}
+
+// ... and the codecs they take: every one with a block compressor, HapA only with an alpha plane
 bool planar_args_ok(const void *alpha, unsigned subsampling, unsigned bitDepth, unsigned colorSpace, unsigned codec, CodecInfo &ci)
 {
-    return subsampling <= HapB200Chroma_444 && (bitDepth == 8 || bitDepth == 10 || bitDepth == 12) && colorSpace <= HapB200YUV_BT709_Full &&
-           codec_info(codec, ci) && codec_encodes(ci) && (ci.bc_kind != kBcRgtc1 || alpha);
+    return planar_format_ok(subsampling, bitDepth, colorSpace) && codec_info(codec, ci) && codec_encodes(ci) && (ci.bc_kind != kBcRgtc1 || alpha);
 }
+
+// BC7 from a Y'CbCr picture encodes the RGBA8 picture made of it (launch_bc7_from_yuv), so that picture's rows, 4 * width
+// bytes, must be rows the RGBA8 encoders take
+bool bc7_rgba_width_ok(unsigned width) { return 4ul * width <= HAPB200_MAX_ROW_BYTES; }
 
 // Hap1 and HapY do not read alpha; HapA reads alpha alone (the picture's other planes are the alpha plane, never read)
 PictureSrc planar_picture(const CodecInfo &ci, const void *luma, const void *cb, const void *cr, const void *alpha, unsigned long chromaPitch,
@@ -2021,6 +2082,71 @@ unsigned int HapB200BlockEncodePlanarBatch(const void *luma, const void *cb, con
 {
     CodecInfo ci;
     if (!planar_args_ok(alpha, subsampling, bitDepth, colorSpace, codec, ci)) return HapResult_Bad_Arguments;
+    return block_encode_picture_batch(ci, planar_picture(ci, luma, cb, cr, alpha, chromaPitch, subsampling, bitDepth, colorSpace), frames,
+                                      frameStride, width, height, lumaPitch, blocks, blocksStride, stream);
+}
+
+// ---- NV12 / P010 and planar Y'CbCr (+ alpha) -> Hap R: the picture encoders with a YUV or planar source and the Hap7 codec;
+// launch_block_encode converts to RGBA8, then runs the RGBA8 BC7 kernel (launch_bc7_from_yuv) ------------------------------
+
+unsigned int HapB200EncodeYUVBC7(const void *luma, const void *chroma, unsigned int width, unsigned int height, unsigned long pitch,
+                                 unsigned int layout, unsigned int colorSpace, unsigned int compressor, unsigned int chunkCount,
+                                 void *outputBuffer, unsigned long outputBufferBytes, unsigned long *outputBufferBytesUsed)
+{
+    if (!yuv_format_ok(layout, colorSpace) || !bc7_rgba_width_ok(width)) return HapResult_Bad_Arguments;
+    return encode_picture(bc7_codec(), yuv_picture(luma, chroma, layout, colorSpace), width, height, pitch, compressor, chunkCount, outputBuffer,
+                          outputBufferBytes, outputBufferBytesUsed);
+}
+
+unsigned int HapB200EncodeYUVBC7Batch(const void *luma, const void *chroma, unsigned int frames, unsigned long frameStride, unsigned int width,
+                                      unsigned int height, unsigned long pitch, unsigned int layout, unsigned int colorSpace,
+                                      unsigned int compressor, unsigned int chunkCount, void *out, unsigned long outStride,
+                                      unsigned long long *used, void *stream)
+{
+    if (!yuv_format_ok(layout, colorSpace) || !bc7_rgba_width_ok(width)) return HapResult_Bad_Arguments;
+    return encode_picture_batch(bc7_codec(), yuv_picture(luma, chroma, layout, colorSpace), frames, frameStride, width, height, pitch, compressor,
+                                chunkCount, out, outStride, used, stream);
+}
+
+unsigned int HapB200BlockEncodeYUVBC7Batch(const void *luma, const void *chroma, unsigned int frames, unsigned long frameStride,
+                                           unsigned int width, unsigned int height, unsigned long pitch, unsigned int layout,
+                                           unsigned int colorSpace, void *blocks, unsigned long blocksStride, void *stream)
+{
+    if (!yuv_format_ok(layout, colorSpace) || !bc7_rgba_width_ok(width)) return HapResult_Bad_Arguments;
+    return block_encode_picture_batch(bc7_codec(), yuv_picture(luma, chroma, layout, colorSpace), frames, frameStride, width, height, pitch,
+                                      blocks, blocksStride, stream);
+}
+
+unsigned int HapB200EncodePlanarBC7(const void *luma, const void *cb, const void *cr, const void *alpha, unsigned int width,
+                                    unsigned int height, unsigned long lumaPitch, unsigned long chromaPitch, unsigned int subsampling,
+                                    unsigned int bitDepth, unsigned int colorSpace, unsigned int compressor, unsigned int chunkCount,
+                                    void *outputBuffer, unsigned long outputBufferBytes, unsigned long *outputBufferBytesUsed)
+{
+    if (!planar_format_ok(subsampling, bitDepth, colorSpace) || !bc7_rgba_width_ok(width)) return HapResult_Bad_Arguments;
+    const CodecInfo ci = bc7_codec();
+    return encode_picture(ci, planar_picture(ci, luma, cb, cr, alpha, chromaPitch, subsampling, bitDepth, colorSpace), width, height, lumaPitch,
+                          compressor, chunkCount, outputBuffer, outputBufferBytes, outputBufferBytesUsed);
+}
+
+unsigned int HapB200EncodePlanarBC7Batch(const void *luma, const void *cb, const void *cr, const void *alpha, unsigned int frames,
+                                         unsigned long frameStride, unsigned int width, unsigned int height, unsigned long lumaPitch,
+                                         unsigned long chromaPitch, unsigned int subsampling, unsigned int bitDepth, unsigned int colorSpace,
+                                         unsigned int compressor, unsigned int chunkCount, void *out, unsigned long outStride,
+                                         unsigned long long *used, void *stream)
+{
+    if (!planar_format_ok(subsampling, bitDepth, colorSpace) || !bc7_rgba_width_ok(width)) return HapResult_Bad_Arguments;
+    const CodecInfo ci = bc7_codec();
+    return encode_picture_batch(ci, planar_picture(ci, luma, cb, cr, alpha, chromaPitch, subsampling, bitDepth, colorSpace), frames, frameStride,
+                                width, height, lumaPitch, compressor, chunkCount, out, outStride, used, stream);
+}
+
+unsigned int HapB200BlockEncodePlanarBC7Batch(const void *luma, const void *cb, const void *cr, const void *alpha, unsigned int frames,
+                                              unsigned long frameStride, unsigned int width, unsigned int height, unsigned long lumaPitch,
+                                              unsigned long chromaPitch, unsigned int subsampling, unsigned int bitDepth,
+                                              unsigned int colorSpace, void *blocks, unsigned long blocksStride, void *stream)
+{
+    if (!planar_format_ok(subsampling, bitDepth, colorSpace) || !bc7_rgba_width_ok(width)) return HapResult_Bad_Arguments;
+    const CodecInfo ci = bc7_codec();
     return block_encode_picture_batch(ci, planar_picture(ci, luma, cb, cr, alpha, chromaPitch, subsampling, bitDepth, colorSpace), frames,
                                       frameStride, width, height, lumaPitch, blocks, blocksStride, stream);
 }

@@ -11,7 +11,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 
 HapB200Codec_Hap1, HapB200Codec_Hap5, HapB200Codec_HapY, HapB200Codec_HapM, HapB200Codec_HapA, HapB200Codec_Hap7 = range(6)
 # HapB200Codec_Hap7 ("Hap R", BC7): the codec-taking RGBA encode entry points refuse it with HapResult_Bad_Arguments; the
-# BC7 encoders (encode_rgba_bc7, encode_rgba_bc7_batch, block_encode_bc7_batch) ask for it by name
+# BC7 encoders (encode_rgba_bc7, encode_rgba_bc7_batch, block_encode_bc7_batch; from NV12 / P010 and planar pictures
+# encode_yuv_bc7, encode_planar_bc7 and their batch forms) ask for it by name
 HapB200YUV_NV12, HapB200YUV_P010 = range(2)
 HapB200YUV_BT601_Limited, HapB200YUV_BT601_Full, HapB200YUV_BT709_Limited, HapB200YUV_BT709_Full = range(4)
 # BT.2020: taken only by the HDR10 encoders (encode_yuv_pq, encode_yuv_pq_batch, block_encode_yuv_pq_batch) and decoders
@@ -88,6 +89,18 @@ class HapB200(HapABI):
         L.HapB200EncodeYUVBatch.argtypes = [vp, vp, u, ul, u, u, ul, u, u, u, u, u, vp, ul, vp, vp]
         L.HapB200BlockEncodeYUVBatch.restype = u
         L.HapB200BlockEncodeYUVBatch.argtypes = [vp, vp, u, ul, u, u, ul, u, u, u, vp, ul, vp]
+        L.HapB200EncodeYUVBC7.restype = u
+        L.HapB200EncodeYUVBC7.argtypes = [vp, vp, u, u, ul, u, u, u, u, vp, ul, C.POINTER(ul)]
+        L.HapB200EncodeYUVBC7Batch.restype = u
+        L.HapB200EncodeYUVBC7Batch.argtypes = [vp, vp, u, ul, u, u, ul, u, u, u, u, vp, ul, vp, vp]
+        L.HapB200BlockEncodeYUVBC7Batch.restype = u
+        L.HapB200BlockEncodeYUVBC7Batch.argtypes = [vp, vp, u, ul, u, u, ul, u, u, vp, ul, vp]
+        L.HapB200EncodePlanarBC7.restype = u
+        L.HapB200EncodePlanarBC7.argtypes = [vp, vp, vp, vp, u, u, ul, ul, u, u, u, u, u, vp, ul, C.POINTER(ul)]
+        L.HapB200EncodePlanarBC7Batch.restype = u
+        L.HapB200EncodePlanarBC7Batch.argtypes = [vp, vp, vp, vp, u, ul, u, u, ul, ul, u, u, u, u, u, vp, ul, vp, vp]
+        L.HapB200BlockEncodePlanarBC7Batch.restype = u
+        L.HapB200BlockEncodePlanarBC7Batch.argtypes = [vp, vp, vp, vp, u, ul, u, u, ul, ul, u, u, u, vp, ul, vp]
         L.HapB200EncodePlanar.restype = u
         L.HapB200EncodePlanar.argtypes = [vp, vp, vp, vp, u, u, ul, ul, u, u, u, u, u, u, vp, ul, C.POINTER(ul)]
         L.HapB200EncodePlanarBatch.restype = u
@@ -361,6 +374,49 @@ class HapB200(HapABI):
                                   bit_depth, color_space, codec, blocks, blocks_stride, stream=None):
         return int(self.lib.HapB200BlockEncodePlanarBatch(luma, cb, cr, alpha, frames, frame_stride, w, h, luma_pitch, chroma_pitch,
                                                           subsampling, bit_depth, color_space, codec, blocks, blocks_stride, stream))
+
+    # -- NV12 / P010 and planar Y'CbCr (+ alpha) -> Hap R (BC7): the arguments of encode_yuv* / encode_planar* without the
+    #    codec; exactly the bytes of the RGBA8 BC7 encoders on the converted picture; a planar alpha None means A = 255.
+    #    Frames need max_encoded_length_rgba(w, h, HapB200Codec_Hap7, chunks)
+    def encode_yuv_bc7(self, luma, chroma, w, h, layout, color_space, compressor=1, chunks=1, pitch=None, out=None, out_capacity=None):
+        """luma, chroma: buffer objects or (addr, nbytes).  Returns (result, frame bytes | used)."""
+        from .abi import _as_ptr
+        laddr, _ = _as_ptr(luma)
+        caddr, _ = _as_ptr(chroma)
+        cap = self.max_encoded_length_rgba(w, h, HapB200Codec_Hap7, chunks) if out_capacity is None else out_capacity
+        return self._encode_frame(cap, out, lambda o, n, used: self.lib.HapB200EncodeYUVBC7(
+            laddr, caddr, w, h, pitch or (2 if layout == HapB200YUV_P010 else 1) * w, layout, color_space, compressor, chunks, o, n, used))
+
+    def encode_yuv_bc7_batch(self, luma, chroma, frames, frame_stride, w, h, pitch, layout, color_space, compressor, chunks, out,
+                             out_stride, used, stream=None):
+        return int(self.lib.HapB200EncodeYUVBC7Batch(luma, chroma, frames, frame_stride, w, h, pitch, layout, color_space, compressor,
+                                                     chunks, out, out_stride, used, stream))
+
+    def block_encode_yuv_bc7_batch(self, luma, chroma, frames, frame_stride, w, h, pitch, layout, color_space, blocks, blocks_stride,
+                                   stream=None):
+        return int(self.lib.HapB200BlockEncodeYUVBC7Batch(luma, chroma, frames, frame_stride, w, h, pitch, layout, color_space, blocks,
+                                                          blocks_stride, stream))
+
+    def encode_planar_bc7(self, luma, cb, cr, alpha, w, h, subsampling, bit_depth, color_space, compressor=1, chunks=1,
+                          luma_pitch=None, chroma_pitch=None, out=None, out_capacity=None):
+        """luma, cb, cr, alpha: buffer objects, (addr, nbytes) or None.  Returns (result, frame bytes | used)."""
+        from .abi import _as_ptr
+        addrs = [0 if b is None else _as_ptr(b)[0] for b in (luma, cb, cr, alpha)]
+        lp, cp = self._planar_pitches(w, subsampling, bit_depth, luma_pitch, chroma_pitch)
+        cap = self.max_encoded_length_rgba(w, h, HapB200Codec_Hap7, chunks) if out_capacity is None else out_capacity
+        return self._encode_frame(cap, out, lambda o, n, used: self.lib.HapB200EncodePlanarBC7(
+            *addrs, w, h, lp, cp, subsampling, bit_depth, color_space, compressor, chunks, o, n, used))
+
+    def encode_planar_bc7_batch(self, luma, cb, cr, alpha, frames, frame_stride, w, h, luma_pitch, chroma_pitch, subsampling,
+                                bit_depth, color_space, compressor, chunks, out, out_stride, used, stream=None):
+        return int(self.lib.HapB200EncodePlanarBC7Batch(luma, cb, cr, alpha, frames, frame_stride, w, h, luma_pitch, chroma_pitch,
+                                                        subsampling, bit_depth, color_space, compressor, chunks, out, out_stride, used,
+                                                        stream))
+
+    def block_encode_planar_bc7_batch(self, luma, cb, cr, alpha, frames, frame_stride, w, h, luma_pitch, chroma_pitch, subsampling,
+                                      bit_depth, color_space, blocks, blocks_stride, stream=None):
+        return int(self.lib.HapB200BlockEncodePlanarBC7Batch(luma, cb, cr, alpha, frames, frame_stride, w, h, luma_pitch, chroma_pitch,
+                                                             subsampling, bit_depth, color_space, blocks, blocks_stride, stream))
 
     # -- Hap (every codec but Hap HDR) -> NV12 / P010: layout HapB200YUV_*, color_space BT.601 / BT.709 (no BT.2020); both
     #    planes have the row pitch `pitch` (default: width bytes per sample)

@@ -28,7 +28,8 @@ enum HapB200Codec {
 };
 /* Hap R (Hap7): the codec-taking encoders HapB200EncodeRGBA, HapB200EncodeRGBABatch and HapB200BlockEncodeBatch refuse it
  * with HapResult_Bad_Arguments (a BC7 search costs far more per block than the DXT encoders, so a caller asks for it by
- * name): HapB200EncodeRGBABC7, HapB200EncodeRGBABC7Batch and HapB200BlockEncodeBC7Batch encode it.  HapEncode and
+ * name): HapB200EncodeRGBABC7, HapB200EncodeRGBABC7Batch and HapB200BlockEncodeBC7Batch encode it, and
+ * HapB200Encode{YUV,Planar}BC7* encode it from NV12 / P010 and planar Y'CbCr pictures.  HapEncode and
  * HapB200EncodeBatch wrap BC7 textures that were compressed elsewhere.  The RGBA decoders turn BC7 blocks into RGBA8 exactly as the BPTC specification defines them,
  * reserved blocks (first byte 0) included: those decode to (0, 0, 0, 0) in all 16 texels. */
 
@@ -391,6 +392,57 @@ unsigned int HapB200BlockEncodePlanarBatch(const void *luma, const void *cb, con
                                            unsigned long lumaPitch, unsigned long chromaPitch, unsigned int subsampling,
                                            unsigned int bitDepth, unsigned int colorSpace, unsigned int codec,
                                            void *blocks, unsigned long blocksStride, void *stream);
+
+/* ---- Hap R (BC7, "Hap7") <- NV12 / P010 and planar Y'CbCr 4:2:0 / 4:2:2 / 4:4:4 (+ alpha) ----------------------------------
+ * The BC7 forms of the YUV and planar encoders above, asking for BC7 by name as HapB200EncodeRGBABC7 does: the same
+ * arguments without the codec.  A picture encodes to exactly the bytes HapB200EncodeRGBABC7* / HapB200BlockEncodeBC7Batch
+ * give for the RGBA8 picture made of it by the conversion of HapB200EncodeYUV (NV12 / P010) or of HapB200EncodePlanar
+ * (planar, its alpha rule included).
+ * Alpha: NV12 / P010 give A = 255.  A planar picture's alpha plane is read when it is non-NULL; a NULL alpha means A = 255, and
+ *   then every decoded texel has A = 255 (the BC7 encoder's opaque rule).  There is no alpha-only form: luma, cb and cr are
+ *   always read.
+ * Planes, layouts, subsamplings, depths, colour spaces, geometry and alignment: those of HapB200EncodeYUV* and
+ *   HapB200EncodePlanar*.  In addition, the RGBA8 picture must be one the RGBA8 encoders take: 4 * width <=
+ *   HAPB200_MAX_ROW_BYTES.  BT.2020, unknown layouts, subsamplings, depths or colour spaces, NULL planes and bad geometry are
+ *   refused with HapResult_Bad_Arguments before anything touches the GPU.
+ * Sizes, options: a frame needs HapB200MaxEncodedLengthRGBA(width, height, HapB200Codec_Hap7, chunkCount) bytes
+ *   (outputBufferBytes, outStride); less is refused with HapResult_Buffer_Too_Small.  compressor, chunkCount and the index and
+ *   offset-table options behave as for HapB200EncodeRGBABC7*.
+ * The conversion runs as a pass of its own into device scratch of at most max(4 * width * height, 256 MiB) bytes, whatever
+ * the number of frames; the BC7 search costs orders of magnitude more (DESIGN.md sections 4 and 6). */
+
+/* one picture (host or device pointers) -> one Hap R frame */
+unsigned int HapB200EncodeYUVBC7(const void *luma, const void *chroma, unsigned int width, unsigned int height,
+                                 unsigned long pitch, unsigned int layout, unsigned int colorSpace,
+                                 unsigned int compressor, unsigned int chunkCount,
+                                 void *outputBuffer, unsigned long outputBufferBytes, unsigned long *outputBufferBytesUsed);
+/* frames x picture (device) -> frames x Hap R frame at out + f*outStride, encoded length in used[f] (device) */
+unsigned int HapB200EncodeYUVBC7Batch(const void *luma, const void *chroma, unsigned int frames, unsigned long frameStride,
+                                      unsigned int width, unsigned int height, unsigned long pitch, unsigned int layout,
+                                      unsigned int colorSpace, unsigned int compressor, unsigned int chunkCount,
+                                      void *out, unsigned long outStride, unsigned long long *used, void *stream);
+/* frames x picture (device) -> bare BC7 textures at blocks + f*blocksStride */
+unsigned int HapB200BlockEncodeYUVBC7Batch(const void *luma, const void *chroma, unsigned int frames, unsigned long frameStride,
+                                           unsigned int width, unsigned int height, unsigned long pitch, unsigned int layout,
+                                           unsigned int colorSpace, void *blocks, unsigned long blocksStride, void *stream);
+/* one planar picture (host or device pointers, any alignment, any pitches) -> one Hap R frame */
+unsigned int HapB200EncodePlanarBC7(const void *luma, const void *cb, const void *cr, const void *alpha,
+                                    unsigned int width, unsigned int height, unsigned long lumaPitch, unsigned long chromaPitch,
+                                    unsigned int subsampling, unsigned int bitDepth, unsigned int colorSpace,
+                                    unsigned int compressor, unsigned int chunkCount,
+                                    void *outputBuffer, unsigned long outputBufferBytes, unsigned long *outputBufferBytesUsed);
+/* frames x planar picture (device) -> frames x Hap R frame at out + f*outStride, encoded length in used[f] (device) */
+unsigned int HapB200EncodePlanarBC7Batch(const void *luma, const void *cb, const void *cr, const void *alpha, unsigned int frames,
+                                         unsigned long frameStride, unsigned int width, unsigned int height, unsigned long lumaPitch,
+                                         unsigned long chromaPitch, unsigned int subsampling, unsigned int bitDepth,
+                                         unsigned int colorSpace, unsigned int compressor, unsigned int chunkCount,
+                                         void *out, unsigned long outStride, unsigned long long *used, void *stream);
+/* frames x planar picture (device) -> bare BC7 textures at blocks + f*blocksStride */
+unsigned int HapB200BlockEncodePlanarBC7Batch(const void *luma, const void *cb, const void *cr, const void *alpha, unsigned int frames,
+                                              unsigned long frameStride, unsigned int width, unsigned int height,
+                                              unsigned long lumaPitch, unsigned long chromaPitch, unsigned int subsampling,
+                                              unsigned int bitDepth, unsigned int colorSpace,
+                                              void *blocks, unsigned long blocksStride, void *stream);
 
 /* ---- Hap, Hap Alpha, Hap Q, Hap Q Alpha, Hap Alpha-Only, Hap R -> NV12 / P010------------------------------------------------
  * The decoders write the 4:2:0 pictures a video encoder takes (NVENC surfaces).  The conversion is fused into the block
